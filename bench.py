@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- Mrays/s of the NeuMan ray-marching hot path at 128+128 samples on N B200s.
+"""bench.py -- Mrays/s of the NeuMan ray-marching hot path at 128+128 samples on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Workload (config.workload): render_vanilla -- background NeRF, 1280x720 = 921 600 rays, 128 coarse +
 128 importance samples (the fine net evaluates 256), seeded default-init weights, synthetic camera:
@@ -13,14 +13,17 @@ fixed, so scaling is "strong".
 `value`   : device-resident throughput (rays generated on device, outputs left in HBM).
 `e2e`     : the same metric through the public API that hands back host arrays: camera (host struct) in,
             frame copied device->host inside the timed region.
-`roofline`: the dominant kernel (k_mlp_tc, tcgen05 fp16xfp16->fp32) timed per launch with CUDA events on
+`roofline`: the dominant kernel (k_mlp_tc, wgmma fp16xfp16->fp32) timed per launch with CUDA events on
             its own stream inside the timed region (nm_profile_*), algorithmic FLOPs = evals x 1 186 816.
 `configs` : BASELINE.json configs 2-5 at their stated sizes (device-resident, 1 warm + 2 timed frames each):
             Mrays/s, MLP evaluations, hit rays, MLP TFLOP/s.
-`cpu_baseline` / `--impl reference`: the UNMODIFIED reference's own render_vanilla (baseline/_ref, installed by
-            tools/install_reference.py) on the host cores, on a 64x64-pixel block (4096 rays) of the same frame:
-            1 warm-up + 3 timed runs, median, thread count picked by a short sweep (BASELINE.md §3).  Falls back to the
-            oracle port (kind "port") only when the reference copy is absent.
+`cpu_baseline` / `--impl reference`: the torch-CPU oracle port of the reference's render_vanilla (oracle/neuman_oracle.py,
+            checked against the reference's outputs by tests/test_oracle_vs_reference.py) on the host cores, on a 64x64-pixel
+            block (4096 rays) of the same frame: 1 warm-up + 3 timed runs, median, thread count picked by a short sweep
+            (BASELINE.md §3).
+`--dump-outputs DIR`: after the timed steps, the frame the last device-resident step computed is written as
+            DIR/rgb.npy ([720*1280, 3] float32) and DIR/depth.npy ([720*1280] float32).  The inputs are seeded, so two
+            builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -46,16 +49,12 @@ CPU_WINDOW = (608, 328)            # pixel block of the frame the CPU arm render
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        j = json.load(open(p))
-        return {"tflops_burst": j.get("bf16_tflops"), "tflops_sustained": j.get("bf16_tflops_sustained"),
-                "hbm_gbs": j.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet, dense FP16 / BF16 at a 700 W power limit: a ceiling, not a measured rate
+    return {"tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense fp16, 700 W)"}
 
 
 class ClockSampler:
-    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -76,20 +75,22 @@ class ClockSampler:
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
-        sm, mx, reasons = [], None, set()
+        self.proc.wait()
+        sm, mx, plim, reasons = [], None, None, set()
         for r in self.rows:
             try:
-                sm.append(float(r[0])); mx = float(r[1])
+                sm.append(float(r[0])); mx = float(r[1]); plim = float(r[7])
             except Exception:
                 continue
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
+        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "power_limit_w": plim, "reasons": sorted(reasons),
+                "samples": len(sm)}
 
 
 # -------------------------------------------------------------------------------------------------------------
-# CPU arm: the reference's own functions on the host cores (test infrastructure: oracle/, baseline/_ref)
+# CPU arm: the oracle port of the reference's functions on the host cores (test infrastructure: oracle/)
 # -------------------------------------------------------------------------------------------------------------
 def cpu_model():
     try:
@@ -102,52 +103,26 @@ def cpu_model():
 
 
 class CpuArm:
-    """render_vanilla of the frame's pixel block [x0, x0+w) x [y0, y0+h) on the CPU: the unmodified reference when its copy
-    is importable (kind "reference"), else the oracle port (kind "port")."""
+    """render_vanilla of the frame's pixel block [x0, x0+w) x [y0, y0+h) on the CPU by the oracle port (kind "port")."""
 
     def __init__(self):
+        import neuman_b200 as nb
         from neuman_b200 import synthetic
-        from oracle import ref_import
+        from oracle import neuman_oracle as no
         self.synthetic = synthetic
         self.K, self.c2w = synthetic.camera(H, W, seed=1)
         self.kind = "port"
-        self.ref = None
-        if ref_import.available():
-            try:
-                self.ref = ref_import.load()
-                self.kind = "reference"
-            except Exception as e:                                   # pragma: no cover
-                print(f"bench.py: reference import failed ({e}); timing the oracle port", file=sys.stderr)
-        if self.ref is not None:
-            from oracle import ref_opts
-            self.coarse, self.fine = synthetic.seed_nets(self.ref.vanilla.build_nerf, ref_opts.default_opt(), 1)
-        else:
-            import neuman_b200 as nb
-            from oracle import neuman_oracle as no
-            coarse, fine = synthetic.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False), 1)
-            self.cp, self.fp = no.net_params_from_joiner(coarse), no.net_params_from_joiner(fine)
+        coarse, fine = synthetic.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False), 1)
+        self.cp, self.fp = no.net_params_from_joiner(coarse), no.net_params_from_joiner(fine)
 
     def render(self, x0, y0, w, h):
         """-> (seconds, rgb [h*w,3], depth [h*w])"""
         Kw = self.synthetic.window_camera(self.K, x0, y0)
         torch.set_grad_enabled(False)
         t0 = time.perf_counter()
-        if self.ref is not None:
-            import contextlib
-            import io
-            ref = self.ref
-            cam = ref.pinhole_camera.PinholeCamera(w, h, Kw[0, 0], Kw[1, 1], Kw[0, 2], Kw[1, 2])
-            pose = ref.camera_pose.CameraPose.from_camera_to_world(self.c2w.astype(np.float64))
-            cap = ref.captures.BasePinholeCapture(cam, pose)
-            cap.near, cap.far = {"bkg": 0.0}, {"bkg": 3.14}
-            with contextlib.redirect_stdout(io.StringIO()):
-                rgb, dep = ref.render_utils.render_vanilla(self.coarse, cap, fine_net=self.fine, rays_per_batch=2048,
-                                                           samples_per_ray=S, importance_samples_per_ray=N, return_depth=True)
-            rgb, dep = rgb.reshape(-1, 3), dep.reshape(-1)
-        else:
-            from oracle import neuman_oracle as no
-            rgb, dep = no.render_vanilla(self.cp, self.fp, Kw, self.c2w, h, w, 0.0, 3.14, rays_per_batch=2048,
-                                         samples_per_ray=S, importance_samples_per_ray=N)
+        from oracle import neuman_oracle as no
+        rgb, dep = no.render_vanilla(self.cp, self.fp, Kw, self.c2w, h, w, 0.0, 3.14, rays_per_batch=2048,
+                                     samples_per_ray=S, importance_samples_per_ray=N)
         return time.perf_counter() - t0, rgb, dep
 
     def pick_threads(self):
@@ -182,7 +157,7 @@ class CpuArm:
         n_rays = side * side
         return {"value": n_rays / med / 1e6, "unit": "Mrays/s", "cores": threads, "kind": self.kind,
                 "sample": (f"{side}x{side} pixel block at ({x0},{y0}) of the same 1280x720 frame = {n_rays} rays, 128+128, "
-                           f"{'unmodified reference render_vanilla (baseline/_ref)' if self.kind == 'reference' else 'torch-CPU oracle port'}, "
+                           f"torch-CPU oracle port, "
                            f"1 warm-up + {runs} runs, median {med:.2f} s; {threads} threads of {os.cpu_count()} logical CPUs "
                            f"({cpu_model()}), 16x16-block thread sweep s: {sweep}"),
                 "cpu_model": cpu_model(), "times_s": [round(t, 3) for t in times]}, (x0, y0, side), rgb, dep
@@ -213,6 +188,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the cfg2-5 side measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the frame of the last timed step as DIR/rgb.npy and DIR/depth.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -295,6 +272,10 @@ def main():
     l0 = ctx.launch_count()
     ms_total, frame = timed(step_device, args.steps)
     launches = ctx.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "rgb.npy"), frame[0].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "depth.npy"), frame[1].float().cpu().numpy())
     prof = ctx.profile_read()
     ctx.profile(False)
     clocks = sampler.stop() if sampler else None
@@ -322,28 +303,22 @@ def main():
         mlp_ms_per_launch = prof["mlp_ms"] / max(prof["mlp_launches"], 1)
         flops_per_launch = prof["mlp_evals"] / max(prof["mlp_launches"], 1) * FLOP_PER_EVAL
         achieved = flops_per_launch / (mlp_ms_per_launch * 1e-3) / 1e12 if prof["mlp_ms"] > 0 else None
-        peak = pk["tflops_sustained"]
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "mlp_tc_traffic.json")
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            traffic = tj.get("dram_bytes_per_launch_bench")       # ncu capture of THIS workload's launches (mean of S=128 and S=256)
+        peak = pk["tflops"]
         line = {
             "metric": METRIC, "value": value, "unit": "Mrays/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-            "dtype": "f16 operands x f32 accumulate (tcgen05 kind::f16); f32 elsewhere", "data": "synthetic",
+            "dtype": "f16 operands x f32 accumulate (wgmma); f32 elsewhere", "data": "synthetic",
             "config": {"workload": WORKLOAD, "global_rays_per_step": n_pix, "mlp_evals_per_ray": EVALS_PER_RAY,
                        "parallelism": f"ray-shard x{world}: interleaved 16x16 pixel tiles + 1 all_gather + un-permute kernel", "warmup_frames_run": n_w,
-                       "l2": "per-step working set (raw [32768x256x4] f32 chunks, 3.8 GB/frame) >> 126 MB L2; no flush needed"},
+                       "l2": "per-step working set (raw [32768x256x4] f32 chunks, 3.8 GB/frame) >> 50 MB L2; no flush needed"},
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": (achieved / peak) if achieved else None,
-                         "traffic": traffic, "traffic_unit": "DRAM bytes per launch: ncu dram__bytes_read+write of this workload's two launch shapes (32768 rays x 128 / x 256 samples), mean; algorithmic 20 B/eval mostly stays in L2",
-                         "kernel": "k_mlp_tc<2>", "peak_source": pk["source"] + " bf16_tflops_sustained (fp16 runs at the bf16 rate)",
+                         "kernel": "k_mlp_tc", "peak_source": pk["source"],
                          "mlp_launches": prof["mlp_launches"], "mlp_ms_per_step": prof["mlp_ms"] / args.steps,
                          "mlp_share_of_step": prof["mlp_ms"] / ms_total},
             "e2e": {"value": e2e_val, "unit": "Mrays/s", "h2d_bytes_per_step": 208, "d2h_bytes_per_step": n_pix * 4 * 4,
                     "api": "neuman_b200.render_vanilla(coarse, cap, fine_net=fine, ...) -> numpy rgb [720,1280,3] + depth (reference signature); "
                            "inputs = the capture's K / camera_to_world (208 B host struct), rays are generated on the device"},
-            "gpu_launches": int(launches), "clocks": clocks, "configs": side, "train_step": train,
+            "gpu": torch.cuda.get_device_name(dev), "gpu_launches": int(launches), "clocks": clocks, "configs": side, "train_step": train,
             "human_train_step": human_train,
         }
         if not args.no_cpu_baseline and world == 1:
@@ -539,7 +514,7 @@ def side_configs(nb, render, sharding, scenes, ctx, dev, rank, world, dist, pk):
         out[name] = {"driver": cfg["driver"] + (" render_can=True" if name.endswith("_can") else ""), "frame": f"{Wc}x{Hc}",
                      "samples": f"{Sc}+{Nc}", "ms_per_frame": ms, "Mrays_s": Hc * Wc / ms / 1e3, "mlp_evals": int(evals),
                      "hit_rays": int(hits), "mlp_ms": mlp_ms, "mlp_tflops_per_gpu": tf,
-                     "mlp_frac_of_peak": tf / pk["tflops_sustained"] if tf else None,
+                     "mlp_frac_of_peak": tf / pk["tflops"] if tf else None,
                      "non_mlp_share": 1.0 - mlp_ms / ms if ms > 0 else None,
                      "per_rank_render_ms": busy, "per_rank_hit_rays": hit_per_rank}
     return out

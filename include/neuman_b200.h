@@ -1,5 +1,5 @@
 /*
- * neuman_b200.h -- C ABI of the B200-native NeuMan ray-marching path.
+ * neuman_b200.h -- C ABI of the H100-native NeuMan ray-marching path.
  *
  * The reference (apple/ml-neuman) is one Python process with no plugin/FFI layer (SURVEY.md §8b);
  * the drop-in boundary is the set of Python functions listed below.  This header declares the
@@ -50,7 +50,7 @@ enum { NM_MLP_TC_F16 = 0, NM_MLP_SIMT_F32 = 1 };
 int nm_ctx_create(int device, nm_ctx** out);
 int nm_ctx_destroy(nm_ctx* ctx);
 const char* nm_last_error(const nm_ctx* ctx);
-/* library build id + the SM architecture the kernels were compiled for ("sm_100a") */
+/* library build id + the SM architecture the kernels were compiled for ("sm_90a") */
 const char* nm_version(void);
 /* number of kernels this library launched on ctx since creation (bench.py's gpu_launches) */
 int64_t nm_launch_count(const nm_ctx* ctx);

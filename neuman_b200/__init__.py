@@ -1,4 +1,4 @@
-"""neuman_b200 -- B200-native (sm_100a) implementation of NeuMan's ray-marching hot path behind the
+"""neuman_b200 -- H100-native (sm_90a) implementation of NeuMan's ray-marching hot path behind the
 reference's own function / module signatures.  See DESIGN.md and INTEGRATION.md.
 
     import neuman_b200 as nb

@@ -108,7 +108,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -m neuman_b200.build` "
-                "(nvcc, sm_100a). neuman_b200 has no CPU fallback.")
+                "(nvcc, sm_90a). neuman_b200 has no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)            # AttributeError if the symbol is not exported

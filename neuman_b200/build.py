@@ -1,4 +1,4 @@
-"""Builds libneuman_b200.so (the C-ABI library) in-tree with nvcc for sm_100a.
+"""Builds libneuman_b200.so (the C-ABI library) in-tree with nvcc for sm_90a (H100).
 
     python -m neuman_b200.build [--force]
 
@@ -30,7 +30,7 @@ SOURCES = {           # file -> extra flags
     "mlp_tc_bwd.cu": [],
     "dw_gemm.cu": [],
 }
-COMMON = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+COMMON = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
           "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 
@@ -72,7 +72,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed")
     if force or procs or _stale(OUT, objs):
-        cmd = [nvcc(), "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [nvcc(), "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         subprocess.check_call(cmd)
     return OUT
 

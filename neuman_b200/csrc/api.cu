@@ -4,7 +4,7 @@
 
 #include "nm_internal.cuh"
 
-extern "C" const char* nm_version(void) { return "neuman_b200 0.1 (sm_100a)"; }
+extern "C" const char* nm_version(void) { return "neuman_b200 0.1 (sm_90a)"; }
 
 extern "C" int nm_ctx_create(int device, nm_ctx** out) {
   if (!out) return NM_ERR_INVALID;
@@ -30,7 +30,6 @@ static void free_net(NmNet& n) {
   if (n.f32) cudaFree(n.f32);
   if (n.f16) cudaFree(n.f16);
   if (n.tc_bias) cudaFree(n.tc_bias);
-  if (n.consts_host) cudaFreeHost(n.consts_host);
   if (n.f16_bwd) cudaFree(n.f16_bwd);
   if (n.bw_wrgb) cudaFree(n.bw_wrgb);
   n = NmNet();

@@ -3,27 +3,28 @@
 // (what torch autograd's  grad_output.t() @ input  computes for every nn.Linear of NeRF.forward,
 // models/vanilla.py:120-152, inside trainers/vanilla_nerf_trainer.py:222 loss.backward()).
 //
-// Both operands are read exactly once, straight from their row-major [n][width] planes:
+// Both operands are read straight from their row-major [n][width] planes:
 //   TMA tensor loads bring 64-row x 64-column boxes into SWIZZLE_128B shared memory; a row-major [rows][64] box
-//   is the canonical *MN-major* UMMA operand (rows = K, columns = M or N), so G serves as A (M = output channel)
-//   and X as B (N = input channel) of tcgen05.mma.cta_group::2.kind::f16 without any transpose.
-//   D[256 x 256] fp32 stays in TMEM while a CTA pair streams its row range; the epilogue reduces the partial
-//   results of the pairs with red.global.add.v4.f32 into the zero-initialised output.
+//   is the canonical *MN-major* GMMA operand (rows = K, columns = M or N), so G serves as A (M = output channel)
+//   and X as B (N = input channel) of wgmma without any transpose in memory.
+//   A CTA owns 128 output channels (two warpgroups of M = 64) x 256 input channels of one GEMM; D[64 x 256] fp32 stays
+//   in each warpgroup's registers while the CTA streams its row range; the epilogue reduces the partial results of the
+//   CTAs with red.global.add.v2.f32 into the zero-initialised output.
 // The nine 256-wide GEMMs of a step (pts_linears 1..7, feature_linear, views_linears.0's feature columns) are
-// one launch: every CTA pair owns one (GEMM, row range) work item sized by its bytes.
-// Bias gradients ride along: one extra N = 16 MMA per K step multiplies G^T with a block of ones, so column 256 of
-// the accumulator holds sum_rows G[row][m] (rows past n are zero-filled by TMA and add nothing).
+// one launch: every pair of CTAs (the two output-channel halves) owns one (GEMM, row range) work item sized by its bytes.
+// Bias gradients ride along: one extra N = 16 MMA per K step multiplies G^T with a block of ones, so every column of
+// that accumulator holds sum_rows G[row][m] (rows past n are zero-filled by TMA and add nothing).
 #include "nm_internal.cuh"
 #include "tc_common.cuh"
 #include <string.h>
 
-#define DW_STAGES 6
+#define DW_STAGES 4
 #define DW_ROWS 64                          // K rows per pipeline stage
 #define DW_BOX_BYTES (DW_ROWS * 128)        // one 64-column box
-#define DW_STAGE_BYTES (4 * DW_BOX_BYTES)   // A: 2 boxes (this CTA's 128 M columns), B: 2 boxes (its 128 N columns)
+#define DW_STAGE_BYTES (6 * DW_BOX_BYTES)   // A: 2 boxes (this CTA's 128 M columns), B: 4 boxes (256 N columns)
 #define DW_MAX_WORK 74
 #define DW_ITEMS 9
-#define DW_THREADS 192                      // producer warp, MMA/relay warp, 4 epilogue warps
+#define DW_THREADS 256                      // two consumer warpgroups
 
 struct DwWork {
   int a_map, a_plane, b_map, b_plane, out_idx, m_rows;
@@ -41,10 +42,9 @@ struct DwCfg {
   static constexpr int OFF_STAGE = 0;
   static constexpr int OFF_ONES = DW_STAGES * DW_STAGE_BYTES;     // one box of fp16 1.0 (any operand layout reads ones)
   static constexpr int OFF_BAR = OFF_ONES + DW_BOX_BYTES;
-  static constexpr int N_BAR = 3 * DW_STAGES + 1;             // full peer_full empty | tmem_full
-  static constexpr int OFF_TMEMPTR = OFF_BAR + 8 * N_BAR;
-  static constexpr int SMEM_BYTES = OFF_TMEMPTR + 16 + 1024;  // + alignment slack
+  static constexpr int SMEM_BYTES = OFF_BAR + 16 * DW_STAGES + 1024;  // + alignment slack
 };
+static_assert(DwCfg::SMEM_BYTES <= 232448, "shared memory of the weight-gradient kernel exceeds 227 KB");
 
 __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, int col, int row, int plane, uint32_t bar) {
   asm volatile(
@@ -52,177 +52,90 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap
       "l"(map), "r"(bar), "r"(col), "r"(row), "r"(plane) : "memory");
 }
 
-// MN-major SWIZZLE_128B operand made of 64-column boxes [DW_ROWS rows][128 B]: 8-row groups (K) 1024 B apart
-// (stride byte offset), 64-column atoms (M/N) one box apart (leading byte offset)
-__device__ __forceinline__ uint64_t dw_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(DW_BOX_BYTES >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-
 __global__ void __launch_bounds__(DW_THREADS, 1) k_dw_gemm(const __grid_constant__ DwParams P) {
   using C = DwCfg;
   extern __shared__ uint8_t smem_dyn[];
-  const uint32_t raw_addr = smem_u32(smem_dyn);
-  const uint32_t pad = (1024 - (raw_addr & 1023)) & 1023;
+  const uint32_t pad = (1024 - (smem_u32(smem_dyn) & 1023)) & 1023;
   uint8_t* smem = smem_dyn + pad;
   const uint32_t sbase = smem_u32(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair_id = blockIdx.x >> 1;
-
+  const int wg = threadIdx.x >> 7, wtid = threadIdx.x & 127;
+  const int lane = threadIdx.x & 31, q = lane & 3;
+  const int half = blockIdx.x & 1;                   // output channels [128 half, 128 half + 128) of the work item
+  const int item = blockIdx.x >> 1;
   auto bar_full = [&](int i) { return sbase + C::OFF_BAR + 8 * i; };
-  auto bar_peer = [&](int i) { return sbase + C::OFF_BAR + 8 * (DW_STAGES + i); };
-  auto bar_empty = [&](int i) { return sbase + C::OFF_BAR + 8 * (2 * DW_STAGES + i); };
-  const uint32_t bar_tfull = sbase + C::OFF_BAR + 8 * (3 * DW_STAGES);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + C::OFF_TMEMPTR);
+  auto bar_empty = [&](int i) { return sbase + C::OFF_BAR + 8 * (DW_STAGES + i); };
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < DW_STAGES; ++i) { mbar_init(bar_full(i), 1); mbar_init(bar_peer(i), 1); mbar_init(bar_empty(i), 1); }
-    mbar_init(bar_tfull, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc<2>(smem_u32(tmem_ptr_smem), 512);
-    tmem_relinquish<2>();
-  }
+  const DwWork W = P.work[item < P.n_work ? item : 0];
+  const bool has_work = item < P.n_work && 128 * half < W.m_rows;
+  const int n_stages = has_work ? (int)((W.row1 - W.row0 + DW_ROWS - 1) / DW_ROWS) : 0;
+
   for (int i = threadIdx.x; i < DW_BOX_BYTES / 4; i += DW_THREADS)
     reinterpret_cast<uint32_t*>(smem + C::OFF_ONES)[i] = 0x3C003C00u;      // fp16 {1.0, 1.0}
   fence_async_smem();                                                      // generic-proxy writes -> tensor-core reads
-  tc_fence_before();
+  int prod = 0;                                                            // producer (thread 0): next stage to load
+  auto produce = [&]() {
+    if (prod >= n_stages) return;
+    const int slot = prod % DW_STAGES, gen = prod / DW_STAGES;
+    if (gen > 0) mbar_wait(bar_empty(slot), (gen - 1) & 1);
+    mbar_arrive_expect_tx(bar_full(slot), DW_STAGE_BYTES);
+    const uint32_t dst = sbase + C::OFF_STAGE + slot * DW_STAGE_BYTES;
+    const int row = (int)(W.row0 + (long long)prod * DW_ROWS);
+    const CUtensorMap* ma = &P.maps[W.a_map];
+    const CUtensorMap* mb = &P.maps[W.b_map];
+    for (int b = 0; b < 2; ++b) tma_load_3d(dst + b * DW_BOX_BYTES, ma, 128 * half + 64 * b, row, W.a_plane, bar_full(slot));
+    for (int b = 0; b < 4; ++b) tma_load_3d(dst + (2 + b) * DW_BOX_BYTES, mb, 64 * b, row, W.b_plane, bar_full(slot));
+    ++prod;
+  };
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < DW_STAGES; ++i) { mbar_init(bar_full(i), 1); mbar_init(bar_empty(i), 2); }
+    fence_mbar_init();
+    for (int i = 0; i < DW_STAGES; ++i) produce();
+  }
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  if (n_stages == 0) return;
 
-  const bool has_work = pair_id < P.n_work;
-  const DwWork W = P.work[has_work ? pair_id : 0];
-  const int n_stages = has_work ? (int)((W.row1 - W.row0 + DW_ROWS - 1) / DW_ROWS) : 0;
-
-  if (n_stages > 0) {
-    if (warp == 0) {
-      // =============================== TMA producer ===============================
-      if (lane == 0) {
-        const CUtensorMap* ma = &P.maps[W.a_map];
-        const CUtensorMap* mb = &P.maps[W.b_map];
-        for (int st = 0; st < n_stages; ++st) {
-          const int slot = st % DW_STAGES, gen = st / DW_STAGES;
-          mbar_wait(bar_empty(slot), (gen & 1) ^ 1);
-          mbar_arrive_expect_tx(bar_full(slot), DW_STAGE_BYTES);
-          const uint32_t dst = sbase + C::OFF_STAGE + slot * DW_STAGE_BYTES;
-          const int row = (int)(W.row0 + (long long)st * DW_ROWS);
-          const int col = (int)rank * 128;
-          tma_load_3d(dst, ma, col, row, W.a_plane, bar_full(slot));
-          tma_load_3d(dst + DW_BOX_BYTES, ma, col + 64, row, W.a_plane, bar_full(slot));
-          tma_load_3d(dst + 2 * DW_BOX_BYTES, mb, col, row, W.b_plane, bar_full(slot));
-          tma_load_3d(dst + 3 * DW_BOX_BYTES, mb, col + 64, row, W.b_plane, bar_full(slot));
-        }
-      }
-    } else if (warp == 1) {
-      if (rank == 0) {
-        // =============================== MMA issuer (leader CTA), warp-uniform ===============================
-        uint32_t issuer = 0;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t.reg .b32 r;\n\telect.sync r|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(issuer));
-        // kind::f16, D = f32, A and B MN-major (bits 15, 16), N = 256, M = 256
-        constexpr uint32_t idesc = make_idesc(256, 256) | (1u << 15) | (1u << 16);
-        constexpr uint32_t idesc_ones = make_idesc(256, 16) | (1u << 15) | (1u << 16);
-        const uint64_t ones_desc = dw_desc(sbase + C::OFF_ONES);
-        for (int st = 0; st < n_stages; ++st) {
-          const int slot = st % DW_STAGES, gen = st / DW_STAGES;
-          mbar_wait(bar_full(slot), gen & 1);
-          mbar_wait(bar_peer(slot), gen & 1);
-          tc_fence_after();
-          const uint32_t base = sbase + C::OFF_STAGE + slot * DW_STAGE_BYTES;
-          const uint64_t a_desc = dw_desc(base);
-          const uint64_t b_desc = dw_desc(base + 2 * DW_BOX_BYTES);
-          if (issuer) {
+  float d[128], db[8];
+  const uint64_t ones_desc = gmma_desc_mn(sbase + C::OFF_ONES, DW_BOX_BYTES);
+  for (int st = 0; st < n_stages; ++st) {
+    const int slot = st % DW_STAGES;
+    mbar_wait(bar_full(slot), (st / DW_STAGES) & 1);
+    const uint32_t base = sbase + C::OFF_STAGE + slot * DW_STAGE_BYTES;
+    wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < DW_ROWS / 16; ++kk)       // 16 K rows = two 8-row groups = 2048 B
-            {
-              umma_f16<2>(tmem_base, a_desc + (uint64_t)(kk * 128), b_desc + (uint64_t)(kk * 128), idesc, (st | kk) != 0);
-              umma_f16<2>(tmem_base + 256, a_desc + (uint64_t)(kk * 128), ones_desc, idesc_ones, (st | kk) != 0);
-            }
-            umma_commit<2>(bar_empty(slot));
-            if (st == n_stages - 1) umma_commit<2>(bar_tfull);
-          }
-          __syncwarp();
-        }
-      } else if (lane == 0) {
-        // =============================== relay (peer CTA) ===============================
-        for (int st = 0; st < n_stages; ++st) {
-          const int slot = st % DW_STAGES, gen = st / DW_STAGES;
-          mbar_wait(bar_full(slot), gen & 1);
-          mbar_arrive_cluster(bar_peer(slot), 0);
-        }
-      }
-    } else {
-      // =============================== epilogue: TMEM -> red.global.add ===============================
-      const int quad = warp & 3;
-      const int m = (int)rank * 128 + quad * 32 + lane;                  // output channel of this thread's TMEM lane
-      mbar_wait(bar_tfull, 0);
-      tc_fence_after();
-      const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16);
-      float* orow = P.out + ((size_t)W.out_idx * 256 + m) * 256;
-      uint32_t v0[16], v1[16];
-      tmem_ld16(t_lane, v0);
-#pragma unroll 1
-      for (int c = 0; c < 256; c += 32) {
-        tmem_wait_ld();
-        tmem_ld16(t_lane + c + 16, v1);
-        if (m < W.m_rows) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(orow + c + j), "f"(__uint_as_float(v0[j])),
-                         "f"(__uint_as_float(v0[j + 1])), "f"(__uint_as_float(v0[j + 2])), "f"(__uint_as_float(v0[j + 3])) : "memory");
-        }
-        tmem_wait_ld();
-        if (c + 32 < 256) tmem_ld16(t_lane + c + 32, v0);
-        if (m < W.m_rows) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(orow + c + 16 + j), "f"(__uint_as_float(v1[j])),
-                         "f"(__uint_as_float(v1[j + 1])), "f"(__uint_as_float(v1[j + 2])), "f"(__uint_as_float(v1[j + 3])) : "memory");
-        }
-      }
-      {                                                                  // bias gradient: any of the 16 equal columns
-        uint32_t b4[4];
-        tmem_ld4(t_lane + 256, b4);
-        tmem_wait_ld();
-        if (m < W.m_rows) atomicAdd(P.bias_out + (size_t)W.out_idx * 256 + m, __uint_as_float(b4[0]));
-      }
-      tc_fence_before();
+    for (int kk = 0; kk < DW_ROWS / 16; ++kk) {       // 16 K rows = two 8-row groups = 2048 B
+      const uint64_t a_desc = gmma_desc_mn(base + wg * DW_BOX_BYTES + kk * 2048, DW_BOX_BYTES);
+      const uint64_t b_desc = gmma_desc_mn(base + 2 * DW_BOX_BYTES + kk * 2048, DW_BOX_BYTES);
+      wgmma_n256_mn(d, a_desc, b_desc, (st | kk) != 0);
+      wgmma_n16_mn(db, a_desc, ones_desc, (st | kk) != 0);
+    }
+    wgmma_commit();
+    if (st > 0) {
+      wgmma_wait<1>();
+      if (wtid == 0) mbar_arrive_local(bar_empty((st - 1) % DW_STAGES));
+      if (threadIdx.x == 0) produce();
+      __syncwarp();
     }
   }
+  wgmma_wait<0>();
+  wgmma_fence_regs(d);
+  wgmma_fence_regs(db);
 
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<2>(tmem_base, 512);
+  // ---- epilogue: registers -> red.global.add (rows = output channels m, columns = input channels) ----
+  const int mA = 128 * half + 64 * wg + 16 * (wtid >> 5) + (lane >> 2), mB = mA + 8;
+  float* oA = P.out + ((size_t)W.out_idx * 256 + mA) * 256;
+  float* oB = P.out + ((size_t)W.out_idx * 256 + mB) * 256;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const int c = 8 * j + 2 * q;
+    if (mA < W.m_rows)
+      asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(oA + c), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+    if (mB < W.m_rows)
+      asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(oB + c), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
   }
-}
-
-// [planes][rows][width] fp16 load map, box = 64 columns x DW_ROWS rows
-static int dw_make_load_map(CUtensorMap* map, const void* base, uint64_t planes, uint64_t rows, uint32_t width) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn) return -1;
-    encode = reinterpret_cast<EncodeFn>(fn);
+  if (q == 0) {                                                      // bias gradient: any of the 16 equal columns
+    if (mA < W.m_rows) atomicAdd(P.bias_out + (size_t)W.out_idx * 256 + mA, db[0]);
+    if (mB < W.m_rows) atomicAdd(P.bias_out + (size_t)W.out_idx * 256 + mB, db[2]);
   }
-  const cuuint64_t dims[3] = {width, rows, planes};
-  const cuuint64_t strides[2] = {(cuuint64_t)width * 2, (cuuint64_t)rows * width * 2};
-  const cuuint32_t box[3] = {64, DW_ROWS, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
 int nm_impl_dw_gemm(nm_ctx* ctx, const __half* g_pre, const __half* g_f, const __half* g_v, const __half* st_x,
@@ -232,13 +145,14 @@ int nm_impl_dw_gemm(nm_ctx* ctx, const __half* g_pre, const __half* g_f, const _
   NM_CHECK_CUDA(ctx, cudaMemsetAsync(bias_out, 0, (size_t)DW_ITEMS * 256 * sizeof(float), st));
   DwParams P;
   memset(&P, 0, sizeof(P));
-  if (dw_make_load_map(&P.maps[0], g_pre, 8, (uint64_t)n, 256) || dw_make_load_map(&P.maps[1], g_f, 1, (uint64_t)n, 256) ||
-      dw_make_load_map(&P.maps[2], g_v, 1, (uint64_t)n, 128) || dw_make_load_map(&P.maps[3], st_x, 8, (uint64_t)n, 256) ||
-      dw_make_load_map(&P.maps[4], st_f, 1, (uint64_t)n, 256))
+  const CUtensorMapL2promotion l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
+  if (tc_make_map(&P.maps[0], g_pre, 8, (uint64_t)n, 256, DW_ROWS, l2) || tc_make_map(&P.maps[1], g_f, 1, (uint64_t)n, 256, DW_ROWS, l2) ||
+      tc_make_map(&P.maps[2], g_v, 1, (uint64_t)n, 128, DW_ROWS, l2) || tc_make_map(&P.maps[3], st_x, 8, (uint64_t)n, 256, DW_ROWS, l2) ||
+      tc_make_map(&P.maps[4], st_f, 1, (uint64_t)n, 256, DW_ROWS, l2))
     NM_FAIL(ctx, NM_ERR_CUDA, "nm_dw_gemm: cuTensorMapEncodeTiled failed");
   P.out = out;
   P.bias_out = bias_out;
-  // work items: item k < 7 = pts_linears k+1 (G plane k+1, X plane k), 7 = feature_linear (g_f, X plane 7),
+  // work items (two CTAs each, one per half of the output channels): item k < 7 = pts_linears k+1 (G plane k+1, X plane k), 7 = feature_linear (g_f, X plane 7),
   // 8 = views_linears.0 feature columns (g_v: 128 output channels, st_f)
   int pairs_total = ctx->sm_count / 2;
   if (pairs_total > DW_MAX_WORK) pairs_total = DW_MAX_WORK;
@@ -271,17 +185,7 @@ int nm_impl_dw_gemm(nm_ctx* ctx, const __half* g_pre, const __half* g_f, const _
   }
   P.n_work = w;
   NM_SET_SMEM_ONCE(ctx, (k_dw_gemm), DwCfg::SMEM_BYTES);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * w);
-  cfg.blockDim = dim3(DW_THREADS);
-  cfg.dynamicSmemBytes = DwCfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NM_CHECK_CUDA(ctx, cudaLaunchKernelEx(&cfg, k_dw_gemm, P));
-  NM_LAUNCHED(ctx);
+  k_dw_gemm<<<2 * w, DW_THREADS, DwCfg::SMEM_BYTES, st>>>(P);
+  NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }

@@ -1,29 +1,23 @@
 // Tensor-core implementation of Joiner.forward (positional encoding + 8x256 NeRF MLP,
-// models/vanilla.py:82-92,:120-152,:162-166) for sm_100a: tcgen05.mma (kind::f16, fp16 operands,
-// fp32 accumulation in TMEM), weights streamed by bulk-TMA (cp.async.bulk) through a shared-memory
-// ring, activations kept on chip between layers, warp-specialised roles, persistent CTAs.
+// models/vanilla.py:82-92,:120-152,:162-166) for sm_90a: wgmma (fp16 operands from shared memory, fp32
+// accumulators in registers), weights streamed by bulk-TMA (cp.async.bulk) through a shared-memory ring,
+// activations kept on chip between layers, persistent CTAs.
 //
 // fp16 operands carry the same 11-bit significand as TF32, at twice the tensor rate; accumulation,
 // bias, ReLU, the alpha head and the encodings are fp32 (DESIGN.md "Numerics").
 //
 // Work decomposition
-//   tile      = 128 consecutive samples per CTA (one TMEM lane per sample).  With kPair == 2 two
-//               CTAs of a cluster form a cta_group::2 pair: one 256-sample pair-tile, each CTA owns
-//               128 rows of A / D and HALF of every weight slab (N/2 rows of B).
+//   tile      = 128 consecutive samples per CTA, 64 per consumer warpgroup (wgmma M = 64).  The two warpgroups
+//               share every weight slab; each has its own activation buffer and encodings.
 //   step      = one GEMM of the network: 0: L0 (K=64 PE) | 1-4: L1-4 | 5: L5 (PE block + 4 act
 //               blocks, "input first", :131) | 6,7: L6,L7 (+alpha head in the epilogue of 7, :135) |
 //               8: feature (:136) | 9: views layer (4 feature blocks + dir-PE block, N=128, :137-141) |
 //               10: rgb (N=16, 3 used, :143).
-//   slab      = one 64-wide K block of one step's weights for this CTA: [N_cta rows][128 B],
-//               128B-swizzled, K-major -- exactly the UMMA canonical layout, pre-packed in HBM so one
-//               cp.async.bulk moves it.  Slabs flow through an NSLOT-deep ring; with two tiles in
-//               flight a slab is consumed by tile A then tile B before its slot is released.
-//   warps     : 0 = bulk-TMA producer, 1 = TMEM allocator + MMA issuer (leader CTA) / relay (peer),
-//               2.. = epilogue warpgroups (one per tile in flight; thread == sample row).
-//   epilogue  : tcgen05.ld 32 columns -> +bias -> ReLU -> cvt to f16x2 -> swizzled st.shared into the
-//               tile's activation buffer, which is the next step's A operand (in place).
-//   on-chip   : act[NT][4 kblocks][128][128B] + one PE block shared by the tiles (the encodings live
-//               in the epilogue threads' registers and are written to it just before steps 0/5/9).
+//   slab      = one 64-wide K block of one step's weights: [N rows][128 B], 128B-swizzled, K-major -- the GMMA
+//               canonical layout, pre-packed in HBM so one cp.async.bulk moves it.  Slabs flow through a
+//               TC_NSLOT-deep ring (tc_common.cuh: TcRing).
+//   epilogue  : accumulator registers -> ReLU -> cvt to f16x2 -> swizzled st.shared into the warpgroup's
+//               activation buffer, which is the next step's A operand (in place).
 #include "nm_internal.cuh"
 #include "nm_pe.cuh"
 #include "tc_common.cuh"
@@ -32,78 +26,56 @@
 // Plan: which slabs a step consumes, where they live in the packed image.
 // ---------------------------------------------------------------------------------------------
 struct TcPlan {
-  uint32_t slab_off[TC_STEPS][5];   // byte offset inside one CTA-rank image
-  uint32_t slab_bytes[TC_STEPS];    // bytes per slab of this step (per CTA)
-  uint32_t image_bytes;             // size of one CTA-rank image
+  uint32_t slab_off[TC_STEPS][5];   // byte offset inside the image
+  uint32_t slab_bytes[TC_STEPS];    // bytes per slab of this step
+  uint32_t image_bytes;             // size of the image
 };
 
 // Every layer's bias rides in the MMAs.  The last channel of each encoding is the constant 1 (channel 63 of the position
 // encoding, 27 of the direction encoding) and the weight column that multiplies it holds the bias (fp16, like every other
-// weight): steps 0, 5 and 9 read the PE block anyway, so there the bias costs nothing.  The K = 256 steps (1-4, 6-8) get
-// one extra k-block, a "bias slab" that is zero except for column 63, consumed by ONE K = 16 MMA against the last K slice
-// (channels 48..63) of whatever encoding the PE block holds at that moment: channels 48..62 meet zero weights, channel 63
-// is 1 in every position encoding, and the direction-encoding stores never touch that half of the block.  The epilogue
-// then has no bias loads and no adds at all -- they were its largest cost (4 LDS.128 broadcasts + 16 FADD per 16 columns
-// on the pipe that also feeds the UMMA operands and takes the activation stores: profiles/r02_mlp_tc_experiments.md); the
-// extra MMA costs 1/16 of a layer's tensor time.  (A variant with a 256-byte constant-ones A operand -- K-major without
-// swizzle, zero stride between row groups -- and a hi + lo bias pair in a 4 KB slab computed the right values but ran 10 %
-// slower and dead-locked in multi-round launches; with five slabs per step and a five-slot ring shared by both tiles there
-// is no room for a sixth slab at steps 5 and 9 either.  Not kept.)
+// weight): steps 0, 5 and 9 read an encoding block anyway, so there the bias costs nothing.  The K = 256 steps (1-4, 6-8)
+// get one extra k-block, a "bias slab" that is zero except for column 63, consumed by ONE K = 16 MMA against the last K
+// slice (channels 48..63) of the position encoding: channels 48..62 meet zero weights, channel 63 is 1.  The epilogue then
+// has no bias loads and no adds at all; the extra MMA costs 1/16 of a layer's tensor time.
 __host__ __device__ constexpr int step_nkb(int s) { return s == 0 ? 1 : (s == 10 ? 2 : 5); }
 __host__ __device__ constexpr bool kb_is_bias(int s, int kb) { return kb == 4 && s != 5 && s != 9 && s >= 1 && s <= 8; }
 __host__ __device__ constexpr int step_N(int s) { return s <= 8 ? 256 : (s == 9 ? 128 : 16); }
-// k-block kb of step s reads the PE buffer (else activation block `act_kb`)
-__host__ __device__ constexpr bool kb_is_pe(int s, int kb) { return (s == 0) || (s == 5 && kb == 0) || (s == 9 && kb == 4); }
+// k-block kb of step s reads the position encoding / the direction encoding (else activation block `act_kb`)
+__host__ __device__ constexpr bool kb_is_pos(int s, int kb) { return (s == 0) || (s == 5 && kb == 0) || kb_is_bias(s, kb); }
+__host__ __device__ constexpr bool kb_is_dir(int s, int kb) { return s == 9 && kb == 4; }
 __host__ __device__ constexpr int kb_act_index(int s, int kb) { return s == 5 ? kb - 1 : kb; }
-__host__ __device__ constexpr int kb_ksteps(int s, int kb) { return (s == 9 && kb == 4) ? 2 : 4; }   // dir PE: K=32
+__host__ __device__ constexpr int tc_slabs_per_tile() {
+  int n = 0;
+  for (int s = 0; s < TC_STEPS; ++s) n += step_nkb(s);
+  return n;
+}
 
-template <int kPair>
 struct TcCfg {
-  static constexpr int NT = kPair == 2 ? 2 : 1;
-  static constexpr int NSLOT = kPair == 2 ? 5 : 4;
-  static constexpr int SLOT_BYTES = 32768 / kPair;
-  static constexpr int THREADS = 64 + 256 + 128;  // producer + MMA warps, 8 epilogue warps, 4 encoding warps
-  static constexpr int OFF_ACT = 0;
-  static constexpr int OFF_PE = OFF_ACT + NT * 4 * TC_KB_BYTES;
-  static constexpr int OFF_RING = OFF_PE + TC_KB_BYTES;
-  static constexpr int OFF_BAR = OFF_RING + NSLOT * SLOT_BYTES;
-  // barriers: full[NSLOT] peer_full[NSLOT] empty[NSLOT] tmem_full[NT] act_ready[NT] pe_free pe_ready
-  static constexpr int N_BAR = 3 * NSLOT + 2 * NT + 2;
-  static constexpr int OFF_TMEMPTR = OFF_BAR + 8 * N_BAR;
-  // alpha-head partials of the upper column half, one float per row and tile in flight
-  static constexpr int OFF_ALPHA = (OFF_TMEMPTR + 16 + 127) & ~127;
-  static constexpr int SMEM_USED = OFF_ALPHA + NT * 512;
-  static constexpr int SMEM_SLACK = (232448 - SMEM_USED) < 1024 ? (232448 - SMEM_USED) : 1024;   // alignment slack that still fits 227 KB
-  static constexpr int SMEM_BYTES = SMEM_USED + SMEM_SLACK;
+  static constexpr int THREADS = 256;                  // two consumer warpgroups
+  // per warpgroup: act[4 k-blocks] | position encoding | direction encoding
+  static constexpr int OFF_POS = 4 * TC_KB_BYTES;
+  static constexpr int OFF_DIR = 5 * TC_KB_BYTES;
+  static constexpr int WG_BYTES = 6 * TC_KB_BYTES;
+  static constexpr int OFF_RING = 2 * WG_BYTES;
+  static constexpr int OFF_BAR = OFF_RING + TC_NSLOT * TC_SLAB_BYTES;
+  static constexpr int OFF_CONST = OFF_BAR + 16 * TC_NSLOT;         // the constant table (k_tc_consts), fp32
+  static constexpr int SMEM_USED = OFF_CONST + 4 * TC_CONST_FLOATS;
+  static constexpr int SMEM_BYTES = SMEM_USED + 1024;               // + alignment slack of the 1024-byte swizzle atoms
 };
+static_assert(TcCfg::SMEM_BYTES <= 232448, "shared memory of the forward kernel exceeds 227 KB");
 
-// What the epilogue threads still multiply or add with, the same for every row -- the alpha_linear weights (the alpha
-// head runs in fp32 on the unrounded post-ReLU layer-7 accumulators, models/vanilla.py:135) and the four output biases --
-// is read from a CONSTANT BANK through the uniform datapath (LDCU.128 into uniform registers, then `FFMA R, R, UR, R`): no
-// shared-memory loads (the LSU / shared-memory pipe is the busiest unit of this kernel: UMMA operand fetches + activation
-// stores) and no vector registers.  Inference launches carry the table as kernel parameters (bank 0); the training forward, whose weights are
-// re-packed on the device every optimiser step, reads a __constant__ copy refreshed by a stream-ordered
-// device-to-device copy in front of the launch (filling kernel parameters would need a host round trip per step).
-//   [0, 256) alpha_linear.weight | 256..258 rgb bias | 259 alpha bias
+// constant table of the epilogue: [0, 256) alpha_linear.weight | 256..258 rgb bias | 259 alpha bias
 #define TC_CONST_ALPHA 0
 #define TC_CONST_OUT 256
-__constant__ __align__(16) float c_tc_consts[TC_CONST_FLOATS];
-
-// with two tiles sharing every slab, a step's slabs must all fit the ring at once (see step_nkb)
-__host__ __device__ constexpr bool ring_holds_a_step(int nslot) {
-  for (int s = 0; s < TC_STEPS; ++s)
-    if (step_nkb(s) > nslot) return false;
-  return true;
-}
-static_assert(ring_holds_a_step(TcCfg<2>::NSLOT), "a step has more slabs than the ring has slots: tiles A and B would deadlock");
 
 struct TcParams {
-  const uint8_t* wimg;      // packed slabs, kPair images back to back
+  const uint8_t* wimg;      // packed slabs
   TcPlan plan;
   NmMlpInput in;
   NmPeSpec pos_pe, dir_pe;
   float* raw;
-  long long n_tiles;        // number of (pair-)tiles
+  const float* consts;      // device constant table (TC_CONST_FLOATS)
+  long long n_tiles;        // number of 128-sample tiles
   int32_t* range_flag;      // device word: bit 0 is set when an activation reached the fp16 range limit (saturated)
   int range_phase;          // sampled range check (kRange == 1): the rounds r with r % 64 == range_phase % 64 are checked
   // training forward (kTrain): fp16 activation stash for the backward pass, planes of n rows each
@@ -113,17 +85,7 @@ struct TcParams {
   uint32_t* st_m;           // [9][n][8]   sign words, 16 bits per 16 columns: bit j = [col 2j > 0], bit 8+j = [col 2j+1 > 0];
                             //             planes 0..7 = pts_linears, plane 8 = views layer (words 0..3 used)
   CUtensorMap map_x, map_f, map_v;   // TMA store maps of st_x / st_f / st_v (kTrain only)
-  int dbg;                  // debug (NEUMAN_TC_DEBUG): bit 0 = training kernel skips its TMA stash stores (timing experiments only)
-  long long* trace;         // optional debug timeline (tools/tc_trace.py): [cta<2][role<2][event<4][256] clock64 stamps
-  __align__(16) float consts[TC_CONST_FLOATS];   // inference: the constant table as kernel parameters
 };
-
-template <bool kParam>
-__device__ __forceinline__ float4 cst4(const TcParams& P, int i) {      // i % 4 == 0
-  return kParam ? *reinterpret_cast<const float4*>(&P.consts[i]) : *reinterpret_cast<const float4*>(&c_tc_consts[i]);
-}
-template <bool kParam>
-__device__ __forceinline__ float cst(const TcParams& P, int i) { return kParam ? P.consts[i] : c_tc_consts[i]; }
 
 // sin/cos of 2*pi*f (f in cycles).  The operands of the tensor-core path are fp16 (quantisation 2.4e-4 on a
 // [-1,1] value), so the encodings only need ~1e-5: range reduction is done exactly in "cycles" with a
@@ -183,7 +145,7 @@ __device__ __forceinline__ void encode_f16(const NmPeSpec& pe, const float x[3],
   for (int i = 0; i < 32; ++i) out[i] = pack_f16x2(ch[2 * i], ch[2 * i + 1], false);
 }
 
-// write 64 f16 (one 128-byte row of a K block) with the 128B swizzle
+// write 8 * nchunks f16 of one 128-byte row of a K block with the 128B swizzle
 __device__ __forceinline__ void store_row_swizzled(uint8_t* blk, int row, const uint32_t* v, int nchunks) {
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -194,12 +156,6 @@ __device__ __forceinline__ void store_row_swizzled(uint8_t* blk, int row, const 
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Epilogue of 16 accumulator columns [c0, c0+16) of one row: + bias, the alpha head on step 7 (fp32 FFMAs on the
-// ReLU of the unrounded accumulators), ReLU, saturating f16x2 pack, two swizzled 16-byte stores into the activation
-// block that is the next step's A operand.  c0 is a compile-time constant and `crow` (= step * 256) warp-uniform, so
-// the bias and the alpha weights are uniform-register operands.
-// ---------------------------------------------------------------------------------------------
 template <bool RELU>
 __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
   uint32_t d;
@@ -217,410 +173,210 @@ __device__ __forceinline__ void track_range(uint32_t& rng, uint32_t packed) {
   rng = *reinterpret_cast<const uint32_t*>(&m);
 }
 
-template <bool RELU, bool ALPHA, bool kParam, bool kRange>
-__device__ __forceinline__ uint32_t epi_sub16(const TcParams& P, const uint32_t (&v)[16], int c0, float (&alpha)[4],
-                                          uint8_t* act, int row, uint32_t& rng) {
-  uint32_t packed[8];
+// ---------------------------------------------------------------------------------------------
+// Epilogue of NC accumulator columns of this thread's two rows rA, rA + 8 (columns 8j + 2q, +1: tc_common.cuh):
+// the alpha head on step 7 (fp32 FFMAs on the ReLU of the unrounded accumulators), ReLU, saturating f16x2 pack,
+// swizzled 4-byte stores into the activation block that is the next step's A operand, and the ReLU sign words
+// (word w = columns 32w..32w+31; bits 0-7 / 8-15: even / odd columns of the first 16, bits 16-31 the same for the
+// next 16) as this thread's share, OR-reduced over the quad afterwards.
+// ---------------------------------------------------------------------------------------------
+template <int NC, bool RELU, bool ALPHA, bool SIGNS>
+__device__ __forceinline__ void fwd_epi(const float (&d)[128], uint8_t* act, int rA, int q, const float* s_walpha,
+                                        float (&alpha)[2], uint32_t (&wA)[8], uint32_t (&wB)[8], bool track, uint32_t& rng) {
+  const int rB = rA + 8;
 #pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const float x0 = __uint_as_float(v[4 * g + 0]), x1 = __uint_as_float(v[4 * g + 1]);      // bias included by the MMAs
-    const float x2 = __uint_as_float(v[4 * g + 2]), x3 = __uint_as_float(v[4 * g + 3]);
+  for (int j = 0; j < NC / 8; ++j) {
+    const int c = 8 * j + 2 * q;
+    const float x0 = d[4 * j], x1 = d[4 * j + 1], y0 = d[4 * j + 2], y1 = d[4 * j + 3];
     if (ALPHA) {                                // alpha_linear on the fp32 ReLU output (:135)
-      const float4 w = cst4<kParam>(P, TC_CONST_ALPHA + c0 + 4 * g);
-      alpha[0] = fmaf(fmaxf(x0, 0.f), w.x, alpha[0]);
-      alpha[1] = fmaf(fmaxf(x1, 0.f), w.y, alpha[1]);
-      alpha[2] = fmaf(fmaxf(x2, 0.f), w.z, alpha[2]);
-      alpha[3] = fmaf(fmaxf(x3, 0.f), w.w, alpha[3]);
+      const float2 w = *reinterpret_cast<const float2*>(s_walpha + c);
+      alpha[0] = fmaf(fmaxf(x0, 0.f), w.x, fmaf(fmaxf(x1, 0.f), w.y, alpha[0]));
+      alpha[1] = fmaf(fmaxf(y0, 0.f), w.x, fmaf(fmaxf(y1, 0.f), w.y, alpha[1]));
     }
-    packed[2 * g] = pack2<RELU>(x0, x1);
-    packed[2 * g + 1] = pack2<RELU>(x2, x3);
+    const uint32_t pA = pack2<RELU>(x0, x1), pB = pack2<RELU>(y0, y1);
+    uint8_t* blk = act + (j >> 3) * TC_KB_BYTES;
+    *reinterpret_cast<uint32_t*>(blk + swz_off(rA, c)) = pA;
+    *reinterpret_cast<uint32_t*>(blk + swz_off(rB, c)) = pB;
+    if (track) { track_range<RELU>(rng, pA); track_range<RELU>(rng, pB); }
+    if (SIGNS) {
+      const __half2 zero2 = __float2half2_rn(0.f);
+      const uint32_t mA = __hgt2_mask(*reinterpret_cast<const __half2*>(&pA), zero2);
+      const uint32_t mB = __hgt2_mask(*reinterpret_cast<const __half2*>(&pB), zero2);
+      const int bit = 16 * ((j >> 1) & 1) + 4 * (j & 1) + q;
+      wA[j >> 2] |= ((mA & 1u) << bit) | ((mA >> 16 & 1u) << (bit + 8));
+      wB[j >> 2] |= ((mB & 1u) << bit) | ((mB >> 16 & 1u) << (bit + 8));
+    }
   }
-  if (kRange) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) track_range<RELU>(rng, packed[j]);
-  }
-  uint8_t* blk = act + (c0 >> 6) * TC_KB_BYTES + row * 128;
-  const int ch0 = (c0 & 63) >> 3;
-  *reinterpret_cast<uint4*>(blk + ((ch0 ^ (row & 7)) << 4)) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-  *reinterpret_cast<uint4*>(blk + (((ch0 + 1) ^ (row & 7)) << 4)) = make_uint4(packed[4], packed[5], packed[6], packed[7]);
-  // ReLU sign word of these 16 outputs (training kernel only): bit j = [column c0+2j > 0], bit 8+j = [column
-  // c0+2j+1 > 0].  The INT32 pipe runs at half the FP rate and this epilogue is short of issue slots in the training
-  // kernel, so the compare is a packed-half HSET2 (one per register, FP16 pipe) that yields 0xFFFF per positive half,
-  // and only one LOP3 per register (pick bit j of each half, OR into the word) plus one PRMT remain on the INT pipe.
-  uint32_t acc = 0;
-  const __half2 zero2 = __float2half2_rn(0.f);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const __half2 h = *reinterpret_cast<const __half2*>(&packed[j]);
-    acc |= __hgt2_mask(h, zero2) & ((1u << j) | (1u << (16 + j)));
-  }
-  return __byte_perm(acc, 0u, 0x4420);          // byte 0 = low halves, byte 1 = high halves
 }
 
-// Drains NC accumulator columns [CB, CB + NC) of this thread's TMEM lane into the activation block, fully unrolled
-// (every column offset is a compile-time constant) and software pipelined over 16-column sub-chunks: the tcgen05.ld
-// of sub-chunk i+1 is in flight while sub-chunk i is converted and stored.
-template <bool RELU, bool ALPHA, int CB, int NC, bool kParam, bool kRange>
-__device__ __forceinline__ void epi_step(const TcParams& P, uint32_t t_lane, float (&alpha)[4], uint8_t* act, int row,
-                                         uint4& signs, uint32_t& rng) {
-  uint32_t v0[16], v1[16];
-  tmem_ld16(t_lane + CB, v0);
+// OR of the sign words over the four threads of a quad (they hold the same rows, different columns)
+__device__ __forceinline__ void quad_or(uint32_t (&w)[8]) {
 #pragma unroll
-  for (int q = 0; q < NC / 32; ++q) {
-    const int c = CB + 32 * q;
-    tmem_wait_ld();
-    tmem_ld16(t_lane + c + 16, v1);
-    const uint32_t m0 = epi_sub16<RELU, ALPHA, kParam, kRange>(P, v0, c, alpha, act, row, rng);
-    tmem_wait_ld();
-    if (q + 1 < NC / 32) tmem_ld16(t_lane + c + 32, v0);
-    const uint32_t m1 = epi_sub16<RELU, ALPHA, kParam, kRange>(P, v1, c + 16, alpha, act, row, rng);
-    const uint32_t w = m0 | (m1 << 16);
-    if (q == 0) signs.x = w; else if (q == 1) signs.y = w; else if (q == 2) signs.z = w; else signs.w = w;
+  for (int i = 0; i < 8; ++i) {
+    w[i] |= __shfl_xor_sync(0xffffffffu, w[i], 1);
+    w[i] |= __shfl_xor_sync(0xffffffffu, w[i], 2);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------
-// debug timeline: role 0 = MMA issuer (events 0: operand ready seen, 1: step issued+committed),
-// role 1 = epilogue warp 2 lane 0 (events 0: accumulator ready seen, 1: drained, 2: published); tile 0 only
-#define TC_TRACE(role, ev, idx)                                                                             \
-  do {                                                                                                      \
-    if (P.trace && blockIdx.x < 2 && (idx) < 256) P.trace[((blockIdx.x * 2 + (role)) * 4 + (ev)) * 256 + (idx)] = clock64(); \
-  } while (0)
-
-template <int kPair, bool kTrain, int kRange>
-__global__ void __launch_bounds__(TcCfg<kPair>::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
-  using C = TcCfg<kPair>;
-  constexpr int NT = C::NT, NSLOT = C::NSLOT;
-  constexpr bool kParam = !kTrain;               // where the constant table comes from (see TcParams::consts)
+template <bool kTrain, int kRange>
+__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
+  using C = TcCfg;
+  constexpr int SLABS = tc_slabs_per_tile();
   extern __shared__ uint8_t smem_dyn[];
-  // SWIZZLE_128B atoms need a 1024-byte aligned base (identical in both CTAs of a pair)
-  const uint32_t raw_addr = smem_u32(smem_dyn);
-  const uint32_t pad = (1024 - (raw_addr & 1023)) & 1023;
-  if (pad > C::SMEM_SLACK) __trap();
+  const uint32_t pad = (1024 - (smem_u32(smem_dyn) & 1023)) & 1023;     // SWIZZLE_128B atoms: 1024-byte aligned base
   uint8_t* smem = smem_dyn + pad;
   const uint32_t sbase = smem_u32(smem);
+  const int wg = threadIdx.x >> 7, wtid = threadIdx.x & 127;
+  const int lane = threadIdx.x & 31, q = lane & 3;
+  const int rA = 16 * (wtid >> 5) + (lane >> 2);        // first of this thread's two accumulator rows (rA, rA + 8)
+  uint8_t* wbuf = smem + wg * C::WG_BYTES;
+  const uint32_t wbase = sbase + wg * C::WG_BYTES;
+  float* s_const = reinterpret_cast<float*>(smem + C::OFF_CONST);
+  const TcRing R{sbase + C::OFF_RING, sbase + C::OFF_BAR};
 
-  // warp index broadcast from lane 0: tells the compiler it is warp-uniform, so role branches are uniform branches and
-  // step-dependent constant-bank addresses can live in uniform registers (LDCU / FADD R, R, UR in the epilogue)
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const uint32_t rank = kPair == 2 ? cluster_ctarank() : 0;
-  const long long pair_id = blockIdx.x / kPair;
-  const long long n_pairs = gridDim.x / kPair;
-
-  auto bar_full = [&](int i) { return sbase + C::OFF_BAR + 8 * i; };
-  auto bar_peer = [&](int i) { return sbase + C::OFF_BAR + 8 * (NSLOT + i); };
-  auto bar_empty = [&](int i) { return sbase + C::OFF_BAR + 8 * (2 * NSLOT + i); };
-  auto bar_tfull = [&](int t) { return sbase + C::OFF_BAR + 8 * (3 * NSLOT + t); };
-  auto bar_aready = [&](int t) { return sbase + C::OFF_BAR + 8 * (3 * NSLOT + NT + t); };
-  const uint32_t bar_pefree = sbase + C::OFF_BAR + 8 * (3 * NSLOT + 2 * NT);
-  const uint32_t bar_peready = sbase + C::OFF_BAR + 8 * (3 * NSLOT + 2 * NT + 1);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + C::OFF_TMEMPTR);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(bar_full(i), 1); mbar_init(bar_peer(i), 1); mbar_init(bar_empty(i), 1); }
-    for (int t = 0; t < NT; ++t) { mbar_init(bar_tfull(t), 1); mbar_init(bar_aready(t), 8 * kPair); }
-    mbar_init(bar_pefree, 1);
-    mbar_init(bar_peready, 4 * kPair);
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc<kPair>(smem_u32(tmem_ptr_smem), 512);
-    tmem_relinquish<kPair>();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (kPair == 2) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  const long long tiles_per_round = n_pairs * NT;
-  const long long n_rounds = (P.n_tiles + tiles_per_round - 1) / tiles_per_round;
-  // sample handled by row `r` of this CTA in tile t of a round
-  auto sample_of = [&](long long round, int t, int r) { return (((round * n_pairs + pair_id) * NT + t) * kPair + rank) * 128 + r; };
-  auto valid_of = [&](long long round, int t, int r) {
-    return ((round * n_pairs + pair_id) * NT + t) < P.n_tiles && sample_of(round, t, r) < P.in.n;
+  for (int i = threadIdx.x; i < TC_CONST_FLOATS; i += C::THREADS) s_const[i] = __ldg(P.consts + i);
+  const long long my_tiles = blockIdx.x < P.n_tiles ? (P.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+  const uint32_t total = (uint32_t)(my_tiles * SLABS);
+  // producer state (thread 0): next slab to issue and its (step, k-block)
+  uint32_t pq = 0;
+  int ps = 0, pkb = 0;
+  auto produce = [&]() {
+    if (pq >= total) return;
+    if (pq >= TC_NSLOT) mbar_wait(R.empty(pq), (pq / TC_NSLOT - 1) & 1);
+    const uint32_t bytes = P.plan.slab_bytes[ps];
+    mbar_arrive_expect_tx(R.full(pq), bytes);
+    bulk_g2s(R.slot(pq), P.wimg + P.plan.slab_off[ps][pkb], bytes, R.full(pq));
+    ++pq;
+    if (++pkb == step_nkb(ps)) { pkb = 0; if (++ps == TC_STEPS) ps = 0; }
   };
-  // PE-buffer use index (order of the MMA stream: per round tile0/tile1 at step 0, then at step 5, then at step 9)
-  auto pe_use = [&](long long round, int k, int t) { return (round * 3 + k) * NT + t; };
-
-  if (warp == 0) {
-    // =============================== bulk-TMA producer ===============================
-    if (lane == 0) {
-      const uint8_t* img = P.wimg + (size_t)rank * P.plan.image_bytes;
-      uint32_t q = 0;
-      for (long long round = 0; round < n_rounds; ++round) {
-        for (int s = 0; s < TC_STEPS; ++s) {
-          for (int kb = 0; kb < step_nkb(s); ++kb, ++q) {
-            const uint32_t bytes = P.plan.slab_bytes[s];
-            const uint32_t slot = q % NSLOT, gen = q / NSLOT;
-            mbar_wait(bar_empty(slot), (gen & 1) ^ 1);
-            mbar_arrive_expect_tx(bar_full(slot), bytes);
-            bulk_g2s(sbase + C::OFF_RING + slot * C::SLOT_BYTES, img + P.plan.slab_off[s][kb], bytes, bar_full(slot));
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (rank == 0) {
-      // =============================== MMA issuer (leader CTA) ===============================
-      // The whole warp runs this loop with warp-uniform values (so descriptors stay in uniform registers and
-      // ptxas needs no divergence "waterfall" around UTCHMMA); one elected lane issues the tcgen05 instructions.
-      uint32_t issuer = 0;
-      asm volatile(
-          "{\n\t.reg .pred p;\n\t.reg .b32 r;\n\telect.sync r|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(issuer));
-      uint32_t q0 = 0, nstep = 0;
-      for (long long round = 0; round < n_rounds; ++round) {
-        for (int s = 0; s < TC_STEPS; ++s, ++nstep) {
-          const uint32_t idesc = make_idesc(128 * kPair, step_N(s));
-          const int nkb = step_nkb(s);
-          const int pe_k = s == 0 ? 0 : (s == 5 ? 1 : 2);
-          for (int t = 0; t < NT; ++t) {
-            mbar_wait(bar_aready(t), nstep & 1);          // A operand written, accumulator drained
-            tc_fence_after();
-            if (t == 0 && issuer) TC_TRACE(0, 0, nstep);
-            const uint32_t d_tmem = tmem_base + t * 256 + (s == 10 ? 128 : 0);
-            for (int kb = 0; kb < nkb; ++kb) {
-              const uint32_t q = q0 + kb, slot = q % NSLOT, gen = q / NSLOT;
-              if (t == 0) {
-                mbar_wait(bar_full(slot), gen & 1);
-                if (kPair == 2) mbar_wait(bar_peer(slot), gen & 1);
-                tc_fence_after();
-              }
-              const bool is_pe = kb_is_pe(s, kb), is_bias = kb_is_bias(s, kb);
-              if (is_pe) {                                // encodings written by the encoding warps of both CTAs
-                mbar_wait(bar_peready, (uint32_t)(pe_use(round, pe_k, t) & 1));
-                tc_fence_after();
-              }
-              // (descriptors are computed by the whole warp, outside the elected-lane region: they stay in uniform registers)
-              const uint32_t a_addr = (is_pe || is_bias) ? sbase + C::OFF_PE
-                                                         : sbase + C::OFF_ACT + (t * 4 + kb_act_index(s, kb)) * TC_KB_BYTES;
-              // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
-              // K = 16 MMA on the last K slice (channels 48..63 of the PE block x columns 48..63 of the slab)
-              const uint64_t a_desc = make_desc(a_addr) + (is_bias ? 6 : 0);
-              const uint64_t b_desc = make_desc(sbase + C::OFF_RING + slot * C::SLOT_BYTES) + (is_bias ? 6 : 0);
-              if (issuer) {
-                umma_f16<kPair>(d_tmem, a_desc, b_desc, idesc, kb != 0);
-                if (!is_bias) {
-                  umma_f16<kPair>(d_tmem, a_desc + 2, b_desc + 2, idesc, 1);
-                  if (kb_ksteps(s, kb) == 4) {
-                    umma_f16<kPair>(d_tmem, a_desc + 4, b_desc + 4, idesc, 1);
-                    umma_f16<kPair>(d_tmem, a_desc + 6, b_desc + 6, idesc, 1);
-                  }
-                }
-                if (t == NT - 1) umma_commit<kPair>(bar_empty(slot));      // slab consumed by every tile
-                if (is_pe) umma_commit<kPair>(bar_pefree);                 // PE block may be rewritten
-              }
-              __syncwarp();
-            }
-            if (issuer) {
-              umma_commit<kPair>(bar_tfull(t));                            // accumulator complete
-              if (t == 0) TC_TRACE(0, 1, nstep);
-            }
-            __syncwarp();
-          }
-          q0 += nkb;
-        }
-      }
-    } else {
-      // =============================== relay (peer CTA of a pair) ===============================
-      // tells the leader's MMA thread that this CTA's half of a slab has landed
-      if (lane == 0) {
-        uint32_t q = 0;
-        for (long long round = 0; round < n_rounds; ++round)
-          for (int s = 0; s < TC_STEPS; ++s)
-            for (int kb = 0; kb < step_nkb(s); ++kb, ++q) {
-              const uint32_t slot = q % NSLOT, gen = q / NSLOT;
-              mbar_wait(bar_full(slot), gen & 1);
-              mbar_arrive_cluster(bar_peer(slot), 0);
-            }
-      }
-    }
-  } else if (warp >= 10) {
-    // ========================= encoding warps: one thread per sample row =========================
-    // Embedder.forward (models/vanilla.py:82-92) of the samples, well ahead of the MMAs that read it: the fp16
-    // encodings of both tiles of a round live in these threads' registers and are stored into the (single) PE block
-    // in the order the MMA stream uses it -- tile 0 / tile 1 at step 0, again at step 5 (skip connection, :131), the
-    // direction encoding at step 9 (:137) -- each store waiting for the MMAs of the previous use to retire.
-    const int prow = (warp - 10) * 32 + lane;
-    uint8_t* pebuf = smem + C::OFF_PE;
-    uint32_t pos[NT][32], dir[NT][16];
-    uint32_t rng = 0;
-    auto encode_pos = [&](long long round) {
-#pragma unroll
-      for (int t = 0; t < NT; ++t) {
-        float p[3] = {0.f, 0.f, 0.f}, v[3] = {0.f, 0.f, 0.f};
-        if (valid_of(round, t, prow)) nm_fetch_sample(P.in, sample_of(round, t, prow), p, v);
-        encode_f16(P.pos_pe, p, pos[t], 30);
-        if (kRange) track_range<false>(rng, pos[t][0]), track_range<false>(rng, pos[t][1]);   // raw x, y, z (+ one sine)
-      }
-    };
-    auto encode_dir = [&](long long round) {
-#pragma unroll
-      for (int t = 0; t < NT; ++t) {
-        float p[3] = {0.f, 0.f, 0.f}, v[3] = {0.f, 0.f, 0.f};
-        if (valid_of(round, t, prow)) nm_fetch_sample(P.in, sample_of(round, t, prow), p, v);
-        uint32_t tmp[32];
-        encode_f16(P.dir_pe, v, tmp, 12);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) dir[t][j] = tmp[j];
-        if (kRange) track_range<false>(rng, tmp[0]), track_range<false>(rng, tmp[1]);
-      }
-    };
-    auto put = [&](long long u, const uint32_t* v, int nchunks) {
-      if (u > 0) mbar_wait_backoff(bar_pefree, (uint32_t)((u - 1) & 1), 32);
-      store_row_swizzled(pebuf, prow, v, nchunks);
-      fence_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(bar_peready, 0);
-    };
-    if (n_rounds > 0) encode_pos(0);
-    for (long long round = 0; round < n_rounds; ++round) {
-#pragma unroll
-      for (int t = 0; t < NT; ++t) put(pe_use(round, 0, t), pos[t], 8);
-      encode_dir(round);
-#pragma unroll
-      for (int t = 0; t < NT; ++t) put(pe_use(round, 1, t), pos[t], 8);
-#pragma unroll
-      for (int t = 0; t < NT; ++t) put(pe_use(round, 2, t), dir[t], 4);
-      if (round + 1 < n_rounds) encode_pos(round + 1);
-    }
-    if (kRange && (((rng & 0xFFFFu) >= 0x7BFFu) || ((rng >> 16) >= 0x7BFFu))) atomicOr(P.range_flag, 1);
-  } else {
-    // ========================= epilogue: 8 warps serve the tiles in flight in turn =========================
-    // Both warpgroups drain every tile: warp (2+q) and warp (6+q) share TMEM lane quadrant q and split the
-    // accumulator columns in halves (g = 0 / 1), so a step's epilogue takes half as long.
-    const int ew = warp - 2;                       // 0..7
-    const int g = ew >> 2;                         // column half
-    const int quad = warp & 3;                     // TMEM lane quadrant this warp may access
-    const int row = quad * 32 + lane;              // sample row inside the CTA tile
-    const int etid = ew * 32 + lane;               // 0..255
-    float* s_alpha = reinterpret_cast<float*>(smem + C::OFF_ALPHA);        // [NT][128] alpha partial of the g==1 half
-    uint32_t nstep = 0;
-    uint32_t rng = 0;
-
-    auto publish = [&](int t) {                     // tile t: A operand ready + accumulator drained
-      fence_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(bar_aready(t), 0);
-    };
-
-    for (long long round = 0; round < n_rounds; ++round) {
-      // ---- step 0 reads only the PE block: nothing to drain, the tiles' accumulators are free ----
-#pragma unroll
-      for (int t = 0; t < NT; ++t) publish(t);
-      float alpha[NT][4];
-#pragma unroll
-      for (int t = 0; t < NT; ++t) alpha[t][0] = alpha[t][1] = alpha[t][2] = alpha[t][3] = 0.f;
-      const long long rperiod = n_rounds < 64 ? n_rounds : 64;
-      const bool track = kRange == 2 || (kRange == 1 && (round % rperiod) == (P.range_phase % rperiod));
-      for (int s = 0; s < TC_STEPS; ++s, ++nstep) {
-#pragma unroll
-        for (int t = 0; t < NT; ++t) {
-          uint8_t* act = smem + C::OFF_ACT + t * 4 * TC_KB_BYTES;
-          const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16) + t * 256;
-          mbar_wait(bar_tfull(t), nstep & 1);
-          tc_fence_after();
-          if (t == 0 && etid == 0) TC_TRACE(1, 0, nstep);
-          if (s < 10) {
-            // training: this warp's slice of the tile's activation buffer is the source of the TMA store issued one
-            // step ago: it must have been read before the slice is overwritten (the other tile's store may still fly)
-            if (kTrain) { if (lane == 0) tma_store_wait_read<1>(); __syncwarp(); }
-            uint4 signs = make_uint4(0, 0, 0, 0);
-            // range flag (kRange 0: off, 2: every sample, 1: every 64th round of the launch, the phase rotating from
-            // launch to launch -- the packed-half max costs ~4 % of the kernel when it runs on every sample)
-#define NM_EPI(RELU, ALPHA, CB, NC)                                                                         \
-  do {                                                                                                       \
-    if (track) epi_step<RELU, ALPHA, CB, NC, kParam, true>(P, t_lane, alpha[t], act, row, signs, rng);         \
-    else epi_step<RELU, ALPHA, CB, NC, kParam, false>(P, t_lane, alpha[t], act, row, signs, rng);              \
-  } while (0)
-            if (g == 0) {
-              if (s == 7) NM_EPI(true, true, 0, 128);
-              else if (s == 8) NM_EPI(false, false, 0, 128);
-              else if (s == 9) NM_EPI(true, false, 0, 64);
-              else NM_EPI(true, false, 0, 128);
-            } else {
-              if (s == 7) NM_EPI(true, true, 128, 128);
-              else if (s == 8) NM_EPI(false, false, 128, 128);
-              else if (s == 9) NM_EPI(true, false, 64, 64);
-              else NM_EPI(true, false, 128, 128);
-            }
-#undef NM_EPI
-            if (kTrain && s < 8 && valid_of(round, t, row))
-              reinterpret_cast<uint4*>(P.st_m + ((size_t)s * P.in.n + sample_of(round, t, row)) * 8)[g] = signs;
-            if (kTrain && s == 9 && valid_of(round, t, row))   // views layer: 64 columns per thread -> words 2g, 2g+1 of plane 8
-              reinterpret_cast<uint2*>(P.st_m + ((size_t)8 * P.in.n + sample_of(round, t, row)) * 8)[g] = make_uint2(signs.x, signs.y);
-            if (s == 7 && g == 1) s_alpha[t * 128 + row] = (alpha[t][0] + alpha[t][1]) + (alpha[t][2] + alpha[t][3]);
-            if (t == 0 && etid == 0) TC_TRACE(1, 1, nstep);
-            if (kTrain) {
-              // activation stash: this warp's 32 rows x (128 | 64) columns leave by TMA straight from the swizzled
-              // A buffer.  Steps 0..7: the MMA thread is told first (the store and the next step's MMAs only read the
-              // slice).  Steps 8 and 9 hand the slice to another warp (the column split changes from 128 to 64 per
-              // warpgroup and back), so there the store must have finished reading before anyone goes on.
-              const long long i0 = sample_of(round, t, row) - lane;            // first row of this warp
-              const bool issue = lane == 0 && i0 < P.in.n && !(P.dbg & 1);
-              const uint32_t src = sbase + C::OFF_ACT + t * 4 * TC_KB_BYTES + quad * 32 * 128;
-              if (s < 8) {
-                publish(t);
-                if (issue) {
-                  tma_store_3d(&P.map_x, src + (2 * g) * TC_KB_BYTES, 128 * g, (int)i0, s);
-                  tma_store_3d(&P.map_x, src + (2 * g + 1) * TC_KB_BYTES, 128 * g + 64, (int)i0, s);
-                  tma_store_commit();
-                }
-              } else {
-                fence_async_smem();
-                __syncwarp();
-                if (issue) {
-                  if (s == 8) {
-                    tma_store_3d(&P.map_f, src + (2 * g) * TC_KB_BYTES, 128 * g, (int)i0, 0);
-                    tma_store_3d(&P.map_f, src + (2 * g + 1) * TC_KB_BYTES, 128 * g + 64, (int)i0, 0);
-                  } else {
-                    tma_store_3d(&P.map_v, src + g * TC_KB_BYTES, 64 * g, (int)i0, 0);
-                  }
-                  tma_store_commit();
-                  tma_store_wait_read<0>();
-                }
-                publish(t);
-              }
-            } else {
-              publish(t);
-            }
-            if (t == 0 && etid == 0) TC_TRACE(1, 2, nstep);
-          } else {
-            if (g == 0) {
-              uint32_t v[4];
-              tmem_ld4(t_lane + 128, v);
-              tmem_wait_ld();
-              if (valid_of(round, t, row)) {
-                const float a = (alpha[t][0] + alpha[t][1]) + (alpha[t][2] + alpha[t][3]) + s_alpha[t * 128 + row];
-                const float4 ob = cst4<kParam>(P, TC_CONST_OUT);
-                float4 o = make_float4(__uint_as_float(v[0]) + ob.x, __uint_as_float(v[1]) + ob.y,
-                                       __uint_as_float(v[2]) + ob.z, a + ob.w);
-                reinterpret_cast<float4*>(P.raw)[sample_of(round, t, row)] = o;   // [r,g,b,sigma] (:144)
-              }
-            }
-            tc_fence_before();
-          }
-        }
-      }
-    }
-    if (kRange && (((rng & 0xFFFFu) >= 0x7BFFu) || ((rng >> 16) >= 0x7BFFu))) atomicOr(P.range_flag, 1);
+  if (threadIdx.x == 0) {
+    R.init();
+    for (int i = 0; i < TC_NSLOT; ++i) produce();
   }
-
-  // ---- teardown ----
-  tc_fence_before();
   __syncthreads();
-  if (kPair == 2) cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<kPair>(tmem_base, 512);
+  auto release = [&](uint32_t qq) {
+    if (wtid == 0) mbar_arrive_local(R.empty(qq));
+    if (threadIdx.x == 0) produce();
+    __syncwarp();
+  };
+
+  const float4 ob = *reinterpret_cast<const float4*>(s_const + TC_CONST_OUT);
+  float d[128];
+  float d16[8];
+  uint32_t rng = 0;
+  uint32_t qbase = 0;
+  const long long rperiod = my_tiles < 64 ? my_tiles : 64;
+  for (long long it = 0; it < my_tiles; ++it) {
+    const long long tile = blockIdx.x + it * gridDim.x;
+    const long long row0 = tile * 128 + wg * TC_WG_ROWS;          // first sample of this warpgroup
+    const bool track = kRange == 2 || (kRange == 1 && (it % rperiod) == (P.range_phase % rperiod));
+    // ---- encodings (Embedder.forward, models/vanilla.py:82-92): threads 0-63 position, 64-127 direction of row wtid % 64 ----
+    {
+      const int r = wtid & 63;
+      float p[3] = {0.f, 0.f, 0.f}, v[3] = {0.f, 0.f, 0.f};
+      if (row0 + r < P.in.n) nm_fetch_sample(P.in, row0 + r, p, v);
+      uint32_t e[32];
+      if (wtid < 64) {
+        encode_f16(P.pos_pe, p, e, 30);
+        store_row_swizzled(wbuf + C::OFF_POS, r, e, 8);
+      } else {
+        encode_f16(P.dir_pe, v, e, 12);
+        store_row_swizzled(wbuf + C::OFF_DIR, r, e, 4);
+      }
+      if (kRange && track) { track_range<false>(rng, e[0]); track_range<false>(rng, e[1]); }   // raw x, y, z (+ one sine)
+      fence_async_smem();
+      wg_sync(wg);
+    }
+    float alpha[2] = {0.f, 0.f};
+    for (int s = 0; s < TC_STEPS; ++s) {
+      const int nkb = step_nkb(s);
+      wgmma_fence();
+      for (int kb = 0; kb < nkb; ++kb) {
+        const uint32_t qq = qbase + kb;
+        R.wait_full(qq);
+        const uint32_t a_addr = kb_is_pos(s, kb) ? wbase + C::OFF_POS
+                              : kb_is_dir(s, kb) ? wbase + C::OFF_DIR
+                                                 : wbase + kb_act_index(s, kb) * TC_KB_BYTES;
+        // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
+        // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab)
+        const bool bias = kb_is_bias(s, kb);
+        const int k0 = bias ? 3 : 0, k1 = kb_is_dir(s, kb) ? 2 : 4;
+        const uint64_t a_desc = gmma_desc_k(a_addr), b_desc = gmma_desc_k(R.slot(qq));
+        for (int k = k0; k < k1; ++k) {
+          const uint32_t acc = (kb | (k - k0)) != 0;
+          if (s <= 8) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+          else if (s == 9) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+          else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
+        }
+        wgmma_commit();
+        if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      wgmma_fence_regs(d16);
+      release(qbase + nkb - 1);
+      qbase += nkb;
+      if (s < 10) {
+        // the MMAs of this step read the activation buffer, the stash stores of the previous step still may: both must
+        // be done before the epilogue overwrites it
+        if (kTrain && wtid == 0) tma_store_wait_read();
+        wg_sync(wg);
+        uint32_t wA[8] = {0, 0, 0, 0, 0, 0, 0, 0}, wB[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const float* s_walpha = s_const + TC_CONST_ALPHA;
+        if (s == 7) fwd_epi<256, true, true, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else if (s == 8) fwd_epi<256, false, false, false>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else if (s == 9) fwd_epi<128, true, false, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else fwd_epi<256, true, false, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        fence_async_smem();
+        wg_sync(wg);
+        if (kTrain) {
+          if (wtid == 0) {
+            if (s < 8) tma_store_rows(&P.map_x, wbase, 0, 4, row0, s);
+            else if (s == 8) tma_store_rows(&P.map_f, wbase, 0, 4, row0, 0);
+            else tma_store_rows(&P.map_v, wbase, 0, 2, row0, 0);
+          }
+          if (s != 8) {
+            quad_or(wA);
+            quad_or(wB);
+            const long long iA = row0 + rA, iB = iA + 8;
+            if (s < 8) {
+              uint32_t* m = P.st_m + (size_t)s * P.in.n * 8;
+              if (iA < P.in.n) reinterpret_cast<uint2*>(m + iA * 8)[q] = make_uint2(wA[2 * q], wA[2 * q + 1]);
+              if (iB < P.in.n) reinterpret_cast<uint2*>(m + iB * 8)[q] = make_uint2(wB[2 * q], wB[2 * q + 1]);
+            } else {
+              uint32_t* m = P.st_m + (size_t)8 * P.in.n * 8;
+              if (iA < P.in.n) m[iA * 8 + q] = wA[q];
+              if (iB < P.in.n) m[iB * 8 + q] = wB[q];
+            }
+          }
+        }
+        if (s == 7) {
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            alpha[r] += __shfl_xor_sync(0xffffffffu, alpha[r], 1);
+            alpha[r] += __shfl_xor_sync(0xffffffffu, alpha[r], 2);
+          }
+        }
+      } else {
+        // rgb (columns 0..2: lane q = 0 holds 0, 1; lane q = 1 holds 2) and the alpha head -> raw [r, g, b, sigma] (:144)
+        const float bA = __shfl_down_sync(0xffffffffu, d16[0], 1), bB = __shfl_down_sync(0xffffffffu, d16[2], 1);
+        const long long iA = row0 + rA, iB = iA + 8;
+        if (q == 0 && iA < P.in.n)
+          reinterpret_cast<float4*>(P.raw)[iA] = make_float4(d16[0] + ob.x, d16[1] + ob.y, bA + ob.z, alpha[0] + ob.w);
+        if (q == 0 && iB < P.in.n)
+          reinterpret_cast<float4*>(P.raw)[iB] = make_float4(d16[2] + ob.x, d16[3] + ob.y, bB + ob.z, alpha[1] + ob.w);
+      }
+    }
   }
+  if (kRange && (((rng & 0xFFFFu) >= 0x7BFFu) || ((rng >> 16) >= 0x7BFFu))) atomicOr(P.range_flag, 1);
+  if (kTrain && wtid == 0) tma_store_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------
-// Packing: fp32 nn.Linear weights -> fp16 slabs in the swizzled UMMA layout.
+// Packing: fp32 nn.Linear weights -> fp16 slabs in the swizzled GMMA layout.
 // ---------------------------------------------------------------------------------------------
 struct PackSrc {
   const float* w[8]; const float* feat; const float* views; const float* rgb;
@@ -650,9 +406,8 @@ __device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int 
   return n < 3 ? S.rgb[(size_t)n * 128 + kb * 64 + kk] : 0.f;
 }
 
-__global__ void k_tc_pack(PackSrc S, TcPlan plan, int kpair, __half* __restrict__ out) {
-  // one thread per packed element of one CTA-rank image; grid.y = rank
-  const int rank = blockIdx.y;
+__global__ void k_tc_pack(PackSrc S, TcPlan plan, __half* __restrict__ out) {
+  // one thread per packed element of the image
   const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;      // half index inside the image
   if (e * 2 >= plan.image_bytes) return;
   const uint32_t byte = (uint32_t)(e * 2);
@@ -662,16 +417,14 @@ __global__ void k_tc_pack(PackSrc S, TcPlan plan, int kpair, __half* __restrict_
     for (int k = 0; k < step_nkb(ss); ++k)
       if (byte >= plan.slab_off[ss][k]) { s = ss; kb = k; }
   const uint32_t in_slab = byte - plan.slab_off[s][kb];
-  const int n_cta = step_N(s) / kpair;
-  const int n_local = in_slab >> 7;
+  const int n = in_slab >> 7;
   const int chunk_phys = (in_slab & 127) >> 4;
-  const int chunk = chunk_phys ^ (n_local & 7);                         // undo the 128B swizzle
+  const int chunk = chunk_phys ^ (n & 7);                               // undo the 128B swizzle
   const int kk = chunk * 8 + ((in_slab & 15) >> 1);
-  const int n = rank * n_cta + n_local;
-  out[(size_t)rank * (plan.image_bytes / 2) + e] = __float2half_rn(src_weight(S, s, n, kb, kk));
+  out[e] = __float2half_rn(src_weight(S, s, n, kb, kk));
 }
 
-// the constant table of the epilogue (layout: TcParams::consts)
+// the constant table of the epilogue (layout: TC_CONST_ALPHA / TC_CONST_OUT)
 __global__ void k_tc_consts(const float* rgb_b, const float* alpha_w, const float* alpha_b, float* __restrict__ out) {
   const int i = threadIdx.x;      // 256 threads
   out[TC_CONST_ALPHA + i] = alpha_w[i];
@@ -714,20 +467,11 @@ int nm_tc_encode(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64
   return NM_OK;
 }
 
-static int tc_pair_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("NEUMAN_TC_PAIR");
-    mode = (e && e[0] == '1') ? 1 : 2;
-  }
-  return mode;
-}
-
-static TcPlan make_plan(int kpair) {
+static TcPlan make_plan() {
   TcPlan p{};
   uint32_t off = 0;
   for (int s = 0; s < TC_STEPS; ++s) {
-    p.slab_bytes[s] = (uint32_t)(step_N(s) / kpair) * 128u;
+    p.slab_bytes[s] = (uint32_t)step_N(s) * 128u;
     for (int kb = 0; kb < step_nkb(s); ++kb) { p.slab_off[s][kb] = off; off += p.slab_bytes[s]; }
   }
   p.image_bytes = off;
@@ -737,9 +481,8 @@ static TcPlan make_plan(int kpair) {
 bool nm_tc_available() { return true; }
 
 int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
-  const int kpair = tc_pair_mode();
-  TcPlan plan = make_plan(kpair);
-  const size_t halfs = (size_t)kpair * plan.image_bytes / 2;
+  TcPlan plan = make_plan();
+  const size_t halfs = plan.image_bytes / 2;
   if (!net.f16 || net.f16_halfs != halfs) {
     if (net.f16) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(net.f16)); net.f16 = nullptr; }
     NM_CHECK_CUDA(ctx, cudaMalloc(&net.f16, halfs * sizeof(__half)));
@@ -752,57 +495,38 @@ int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   S.feat = d.feature_w; S.views = d.views_w; S.rgb = d.rgb_w;
   for (int l = 0; l < 8; ++l) S.b[l] = d.pts_b[l];
   S.feat_b = d.feature_b; S.views_b = d.views_b;
-  dim3 grid((unsigned)((plan.image_bytes / 2 + 255) / 256), kpair);
-  k_tc_pack<<<grid, 256, 0, st>>>(S, plan, kpair, net.f16);
+  k_tc_pack<<<(unsigned)((halfs + 255) / 256), 256, 0, st>>>(S, plan, net.f16);
   NM_CHECK_LAUNCH(ctx);
   k_tc_consts<<<1, 256, 0, st>>>(d.rgb_b, d.alpha_w, d.alpha_b, net.tc_bias);
   NM_CHECK_LAUNCH(ctx);
-  net.consts_host_valid = false;        // the host copy (kernel parameters of inference launches) is refreshed lazily
   return NM_OK;
 }
 
-template <int kPair, bool kTrain, int kRange>
+template <bool kTrain, int kRange>
 static int launch_tc(nm_ctx* ctx, const TcParams& P, cudaStream_t st) {
-  using C = TcCfg<kPair>;
-  NM_SET_SMEM_ONCE(ctx, (k_mlp_tc<kPair, kTrain, kRange>), C::SMEM_BYTES);
-  int ctas = ctx->sm_count - (ctx->sm_count % kPair);
-  long long need = P.n_tiles * kPair;                       // CTAs that have work in the first round
-  need = (need + C::NT - 1) / C::NT;
-  if (need < ctas) ctas = (int)((need + kPair - 1) / kPair * kPair);
-  if (ctas < kPair) ctas = kPair;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(ctas);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kPair; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NM_CHECK_CUDA(ctx, cudaLaunchKernelEx(&cfg, k_mlp_tc<kPair, kTrain, kRange>, P));
-  NM_LAUNCHED(ctx);
+  NM_SET_SMEM_ONCE(ctx, (k_mlp_tc<kTrain, kRange>), TcCfg::SMEM_BYTES);
+  long long ctas = ctx->sm_count;
+  if (P.n_tiles < ctas) ctas = P.n_tiles > 0 ? P.n_tiles : 1;
+  k_mlp_tc<kTrain, kRange><<<(unsigned)ctas, TcCfg::THREADS, TcCfg::SMEM_BYTES, st>>>(P);
+  NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }
 
 int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views, const float* origins,
                   const float* dirs, const float* z, int64_t n, int32_t group, float* raw, cudaStream_t st,
                   const NmTrainStash* stash) {
-  const int kpair = tc_pair_mode();
   if (!net.f16 || !net.tc_bias) NM_FAIL(ctx, NM_ERR_STATE, "nm_tc_forward: weights not packed");
   TcParams P;
   P.wimg = reinterpret_cast<const uint8_t*>(net.f16);
-  P.plan = make_plan(kpair);
+  P.plan = make_plan();
   P.in = NmMlpInput{pts, views, origins, dirs, z, (long long)n, group};
   P.pos_pe = NmPeSpec{net.desc.pos_pe_kind, net.desc.pos_n_freqs, net.f32 + net.o_pos_cyc};
   P.dir_pe = NmPeSpec{net.desc.dir_pe_kind, net.desc.dir_n_freqs, net.f32 + net.o_dir_cyc};
   P.raw = raw;
-  P.n_tiles = (n + 128 * kpair - 1) / (128 * kpair);
-  P.trace = nullptr;
-  P.dbg = 0;
+  P.consts = net.tc_bias;
+  P.n_tiles = (n + 127) / 128;
   P.range_flag = ctx->d_counter + NM_RANGE_FLAG_WORD;
   P.range_phase = (int)(ctx->range_seq++ % 64);
-  if (const char* e = getenv("NEUMAN_TC_DEBUG")) P.dbg = atoi(e);
   P.st_x = stash ? stash->x : nullptr; P.st_f = stash ? stash->f : nullptr; P.st_v = stash ? stash->v : nullptr;
   P.st_m = stash ? stash->m : nullptr;
   memset(&P.map_x, 0, 3 * sizeof(CUtensorMap));
@@ -811,26 +535,14 @@ int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
     if (tc_make_store_map(&P.map_x, stash->x, 8, (uint64_t)n, 256) || tc_make_store_map(&P.map_f, stash->f, 1, (uint64_t)n, 256) ||
         tc_make_store_map(&P.map_v, stash->v, 1, (uint64_t)n, 128))
       NM_FAIL(ctx, NM_ERR_CUDA, "nm_mlp_forward_train: cuTensorMapEncodeTiled failed");
-    // training forward: the constant table stays on the device (stream-ordered copy into the __constant__ bank)
-    NM_CHECK_CUDA(ctx, cudaMemcpyToSymbolAsync(c_tc_consts, net.tc_bias, TC_CONST_FLOATS * sizeof(float), 0,
-                                               cudaMemcpyDeviceToDevice, st));
-  } else {
-    if (!net.consts_host_valid) {       // once per (re)pack: the constant table becomes kernel parameters
-      if (!net.consts_host) NM_CHECK_CUDA(ctx, cudaMallocHost(&net.consts_host, TC_CONST_FLOATS * sizeof(float)));
-      NM_CHECK_CUDA(ctx, cudaMemcpyAsync(net.consts_host, net.tc_bias, TC_CONST_FLOATS * sizeof(float), cudaMemcpyDeviceToHost, st));
-      NM_CHECK_CUDA(ctx, cudaStreamSynchronize(st));
-      net.consts_host_valid = true;
-    }
-    memcpy(P.consts, net.consts_host, sizeof(P.consts));
   }
-  if (const char* e = getenv("NEUMAN_TC_TRACE")) P.trace = reinterpret_cast<long long*>(strtoull(e, nullptr, 0));
   // NEUMAN_TC_RANGE: 0 = no range flag, 1 (default) = sampled (every 64th round, rotating phase), 2 = every sample
   static const int range_mode = [] { const char* e = getenv("NEUMAN_TC_RANGE"); return e ? atoi(e) : 1; }();
-#define NM_LAUNCH(TRAIN)                                                                                                  \
-  do {                                                                                                                     \
-    if (range_mode <= 0) return kpair == 2 ? launch_tc<2, TRAIN, 0>(ctx, P, st) : launch_tc<1, TRAIN, 0>(ctx, P, st);       \
-    if (range_mode == 1) return kpair == 2 ? launch_tc<2, TRAIN, 1>(ctx, P, st) : launch_tc<1, TRAIN, 1>(ctx, P, st);       \
-    return kpair == 2 ? launch_tc<2, TRAIN, 2>(ctx, P, st) : launch_tc<1, TRAIN, 2>(ctx, P, st);                            \
+#define NM_LAUNCH(TRAIN)                                                  \
+  do {                                                                    \
+    if (range_mode <= 0) return launch_tc<TRAIN, 0>(ctx, P, st);          \
+    if (range_mode == 1) return launch_tc<TRAIN, 1>(ctx, P, st);          \
+    return launch_tc<TRAIN, 2>(ctx, P, st);                               \
   } while (0)
   if (P.st_x) NM_LAUNCH(true);
   NM_LAUNCH(false);

@@ -1,9 +1,9 @@
 // Backward (input-gradient) chain of NeRF.forward (models/vanilla.py:120-152) on the tensor cores:
-// the adjoint of mlp_tc.cu's training forward, same machinery (tcgen05.mma cta_group::2 kind::f16, fp32
-// TMEM accumulators, bulk-TMA weight ring, persistent CTA pairs, activations kept on chip).
+// the adjoint of mlp_tc.cu's training forward, same machinery (wgmma, fp16 operands, fp32 register
+// accumulators, bulk-TMA weight ring, persistent CTAs of two 64-row warpgroups, activations kept on chip).
 //
 // For every sample row, with g = dL/d raw (4 values) scaled by the loss scale S:
-//   dVpre = (g_rgb @ Wrgb) * [V > 0]                         (epilogue threads, K = 3; [V > 0] from sign words)
+//   dVpre = (g_rgb @ Wrgb) * [V > 0]                         (K = 3, plain FFMAs; [V > 0] from sign words)
 //   b0: dF   = dVpre @ Wviews[:, :256]                        (K = 128)
 //   b1: dX8  = dF @ Wfeature + g_alpha * w_alpha ;  dpre7 = dX8 * [X8 > 0]
 //   b2..b8 (l = 7..1): dX_{l-1} = dpre_l @ W_l[:, -256:] ;   dpre_{l-1} = dX_{l-1} * [X_{l-1} > 0]
@@ -19,360 +19,186 @@
 __host__ __device__ constexpr int bw_nkb(int b) { return b == 0 ? 2 : 4; }
 #define BW_SLABS (2 + 8 * 4)
 
-// rgb_linear.weight as [3][128] for the head (dV = g_rgb @ Wrgb): every thread needs all 384 values, with indices
-// that are compile-time constants after unrolling, so they are folded into the FFMAs as constant-bank operands
-// (read from shared memory this cost 384 LDS per thread and made the head the slowest step of a round: 17k cycles).
-// Copied from the net's packed image before each launch (stream-ordered, device to device).
-__constant__ float c_bw_wrgb[384];
-
-template <int kPair>
 struct BwCfg {
-  static constexpr int NT = 2;
-  static constexpr int NSLOT = kPair == 2 ? 5 : 3;
-  static constexpr int SLOT_BYTES = 32768 / kPair;
-  static constexpr int THREADS = 64 + 256;
-  static constexpr int OFF_ACT = 0;
-  static constexpr int OFF_RING = OFF_ACT + NT * 4 * TC_KB_BYTES;
-  static constexpr int OFF_BAR = OFF_RING + NSLOT * SLOT_BYTES;
-  static constexpr int N_BAR = 3 * NSLOT + 2 * NT;          // full peer_full empty | tmem_full act_ready
-  static constexpr int OFF_TMEMPTR = OFF_BAR + 8 * N_BAR;
-  static constexpr int OFF_CONST = (OFF_TMEMPTR + 16 + 127) & ~127;   // w_alpha[256] fp32
-  static constexpr int SMEM_USED = OFF_CONST + 1024;
+  static constexpr int THREADS = 256;                      // two consumer warpgroups
+  static constexpr int WG_BYTES = 4 * TC_KB_BYTES;          // per warpgroup: act[4 k-blocks]
+  static constexpr int OFF_RING = 2 * WG_BYTES;
+  static constexpr int OFF_BAR = OFF_RING + TC_NSLOT * TC_SLAB_BYTES;
+  static constexpr int OFF_CONST = OFF_BAR + 16 * TC_NSLOT;  // w_alpha[256] | w_rgb[3][128], fp32
+  static constexpr int SMEM_USED = OFF_CONST + 4 * (256 + 384);
   static constexpr int SMEM_BYTES = SMEM_USED + 1024;
 };
+static_assert(BwCfg::SMEM_BYTES <= 232448, "shared memory of the backward kernel exceeds 227 KB");
 
 struct BwParams {
-  const uint8_t* wimg;      // transposed weight slabs, kPair images back to back
-  uint32_t image_bytes;
+  const uint8_t* wimg;      // transposed weight slabs
   const float* d_raw;       // [n][4] fp32 dL/d(r,g,b,sigma)
   const float* scale;       // device scalar: loss scale S (a power of two)
   const float* w_alpha;     // [256] fp32 alpha_linear.weight
+  const float* w_rgb;       // [3][128] fp32 rgb_linear.weight
   const uint32_t* st_m;     // [9][n][8] forward stash: ReLU sign words of pts_linears 0..7 and (plane 8, 4 words) of the views layer
-  __half* g_pre;            // [8][n][256] out: S * dL/d(pre-activation of pts_linears l)
-  __half* g_f;              // [n][256]    out: S * dL/d feature
-  __half* g_v;              // [n][128]    out: S * dL/d(pre-activation of views_linears.0)
   long long n, n_tiles;
-  CUtensorMap map_pre, map_f, map_v;   // TMA store maps of g_pre / g_f / g_v
-  long long* trace;             // optional debug timeline (tools/tc_trace.py bwd): same layout as mlp_tc.cu's
+  CUtensorMap map_pre, map_f, map_v;   // TMA store maps of g_pre [8][n][256] / g_f [n][256] / g_v [n][128]
 };
 
-// 16 accumulator columns [c0, c0+16) of one row: (+ rank-1 alpha term), ReLU mask from sign bits, pack,
+// mask bit of column c = 8j + 2q + e in word j / 4 of a row's sign words (mlp_tc.cu fwd_epi)
+__device__ __forceinline__ bool sign_bit(const uint32_t (&w)[8], int j, int q, int e) {
+  return (w[j >> 2] >> (16 * ((j >> 1) & 1) + 8 * e + 4 * (j & 1) + q)) & 1u;
+}
+
+// 256 accumulator columns of this thread's rows rA, rA + 8: (+ rank-1 alpha term), ReLU mask from sign bits, pack,
 // swizzled store into the next A operand (from where a TMA store takes it to the HBM gradient plane)
 template <bool ALPHA, bool MASK>
-__device__ __forceinline__ void bw_sub16(const uint32_t (&v)[16], int c0, float da, const float* s_walpha, uint32_t mbits,
-                                         uint8_t* act, int row) {
-  float x[16];
+__device__ __forceinline__ void bw_epi(const float (&d)[128], uint8_t* act, int rA, int q, const float* s_walpha, float daA,
+                                       float daB, const uint32_t (&mA)[8], const uint32_t (&mB)[8]) {
 #pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    x[e] = __uint_as_float(v[e]);
-    if (ALPHA) x[e] = fmaf(da, s_walpha[c0 + e], x[e]);          // same address in every lane: a broadcast
-  }
-  if (MASK) {
-    // sign word layout (mlp_tc.cu epi_sub16): bit k < 8 = column 2k, bit 8+k = column 2k+1; tested in bit order so
-    // that the compiler moves them to predicates wholesale (R2P)
-#pragma unroll
-    for (int k = 0; k < 16; ++k)
-      if (!((mbits >> k) & 1u)) x[k < 8 ? 2 * k : 2 * (k - 8) + 1] = 0.f;
-  }
-  uint32_t packed[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) packed[j] = pack_f16x2(x[2 * j], x[2 * j + 1], false);
-  uint8_t* blk = act + (c0 >> 6) * TC_KB_BYTES + row * 128;
-  const int ch0 = (c0 & 63) >> 3;
-  *reinterpret_cast<uint4*>(blk + ((ch0 ^ (row & 7)) << 4)) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-  *reinterpret_cast<uint4*>(blk + (((ch0 + 1) ^ (row & 7)) << 4)) = make_uint4(packed[4], packed[5], packed[6], packed[7]);
-}
-
-// drains 128 accumulator columns [cbase, cbase+128) of this thread's TMEM lane; mask = 128 sign bits
-template <bool ALPHA, bool MASK>
-__device__ __forceinline__ void bw_step(uint32_t t_lane, int cbase, float da, const float* s_walpha, const uint4& mask,
-                                        uint8_t* act, int row) {
-  uint32_t v0[16], v1[16];
-  const uint32_t mw[4] = {mask.x, mask.y, mask.z, mask.w};
-  tmem_ld16(t_lane + cbase, v0);
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int c = cbase + 32 * q;
-    tmem_wait_ld();
-    tmem_ld16(t_lane + c + 16, v1);
-    bw_sub16<ALPHA, MASK>(v0, c, da, s_walpha, mw[q] & 0xffffu, act, row);
-    tmem_wait_ld();
-    if (q < 3) tmem_ld16(t_lane + c + 32, v0);
-    bw_sub16<ALPHA, MASK>(v1, c + 16, da, s_walpha, mw[q] >> 16, act, row);
+  for (int j = 0; j < 32; ++j) {
+    const int c = 8 * j + 2 * q;
+    float x0 = d[4 * j], x1 = d[4 * j + 1], y0 = d[4 * j + 2], y1 = d[4 * j + 3];
+    if (ALPHA) {
+      const float2 w = *reinterpret_cast<const float2*>(s_walpha + c);
+      x0 = fmaf(daA, w.x, x0); x1 = fmaf(daA, w.y, x1);
+      y0 = fmaf(daB, w.x, y0); y1 = fmaf(daB, w.y, y1);
+    }
+    if (MASK) {
+      if (!sign_bit(mA, j, q, 0)) x0 = 0.f;
+      if (!sign_bit(mA, j, q, 1)) x1 = 0.f;
+      if (!sign_bit(mB, j, q, 0)) y0 = 0.f;
+      if (!sign_bit(mB, j, q, 1)) y1 = 0.f;
+    }
+    uint8_t* blk = act + (j >> 3) * TC_KB_BYTES;
+    *reinterpret_cast<uint32_t*>(blk + swz_off(rA, c)) = pack_f16x2(x0, x1, false);
+    *reinterpret_cast<uint32_t*>(blk + swz_off(rA + 8, c)) = pack_f16x2(y0, y1, false);
   }
 }
 
-// debug timeline, as in mlp_tc.cu: role 0 = MMA issuer (0: operand ready seen, 1: step issued + committed), role 1 =
-// epilogue warp 2 lane 0 (0: accumulator ready seen, 1: drained, 2: handed over); tile 0 of CTAs 0 / 1 only
-#define BW_TRACE(role, ev, idx)                                                                             \
-  do {                                                                                                      \
-    if (P.trace && blockIdx.x < 2 && (idx) < 256) P.trace[((blockIdx.x * 2 + (role)) * 4 + (ev)) * 256 + (idx)] = clock64(); \
-  } while (0)
+__device__ __forceinline__ void load_signs(const uint32_t* m, long long i, long long n, uint32_t (&w)[8]) {
+  uint4 a = make_uint4(0, 0, 0, 0), b = a;
+  if (i < n) { a = __ldg(reinterpret_cast<const uint4*>(m + i * 8)); b = __ldg(reinterpret_cast<const uint4*>(m + i * 8) + 1); }
+  w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+}
 
-template <int kPair>
-__global__ void __launch_bounds__(BwCfg<kPair>::THREADS, 1) k_mlp_tc_bwd(const __grid_constant__ BwParams P) {
-  using C = BwCfg<kPair>;
-  constexpr int NT = C::NT, NSLOT = C::NSLOT;
+__global__ void __launch_bounds__(BwCfg::THREADS, 1) k_mlp_tc_bwd(const __grid_constant__ BwParams P) {
+  using C = BwCfg;
   extern __shared__ uint8_t smem_dyn[];
-  const uint32_t raw_addr = smem_u32(smem_dyn);
-  const uint32_t pad = (1024 - (raw_addr & 1023)) & 1023;          // SWIZZLE_128B atoms: 1024-byte aligned base
+  const uint32_t pad = (1024 - (smem_u32(smem_dyn) & 1023)) & 1023;          // SWIZZLE_128B atoms: 1024-byte aligned base
   uint8_t* smem = smem_dyn + pad;
   const uint32_t sbase = smem_u32(smem);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = kPair == 2 ? cluster_ctarank() : 0;
-  const long long pair_id = blockIdx.x / kPair;
-  const long long n_pairs = gridDim.x / kPair;
-
-  auto bar_full = [&](int i) { return sbase + C::OFF_BAR + 8 * i; };
-  auto bar_peer = [&](int i) { return sbase + C::OFF_BAR + 8 * (NSLOT + i); };
-  auto bar_empty = [&](int i) { return sbase + C::OFF_BAR + 8 * (2 * NSLOT + i); };
-  auto bar_tfull = [&](int t) { return sbase + C::OFF_BAR + 8 * (3 * NSLOT + t); };
-  auto bar_aready = [&](int t) { return sbase + C::OFF_BAR + 8 * (3 * NSLOT + NT + t); };
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + C::OFF_TMEMPTR);
+  const int wg = threadIdx.x >> 7, wtid = threadIdx.x & 127;
+  const int lane = threadIdx.x & 31, q = lane & 3;
+  const int rA = 16 * (wtid >> 5) + (lane >> 2);
+  uint8_t* act = smem + wg * C::WG_BYTES;
+  const uint32_t abase = sbase + wg * C::WG_BYTES;
   float* s_walpha = reinterpret_cast<float*>(smem + C::OFF_CONST);
+  float* s_wrgb = s_walpha + 256;
+  const TcRing R{sbase + C::OFF_RING, sbase + C::OFF_BAR};
 
+  s_walpha[threadIdx.x] = __ldg(P.w_alpha + threadIdx.x);
+  for (int i = threadIdx.x; i < 384; i += C::THREADS) s_wrgb[i] = __ldg(P.w_rgb + i);
+  const long long my_tiles = blockIdx.x < P.n_tiles ? (P.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+  const uint32_t total = (uint32_t)(my_tiles * BW_SLABS);
+  uint32_t pq = 0;                                   // producer (thread 0): next slab to issue
+  auto produce = [&]() {
+    if (pq >= total) return;
+    if (pq >= TC_NSLOT) mbar_wait(R.empty(pq), (pq / TC_NSLOT - 1) & 1);
+    mbar_arrive_expect_tx(R.full(pq), TC_SLAB_BYTES);
+    bulk_g2s(R.slot(pq), P.wimg + (size_t)(pq % BW_SLABS) * TC_SLAB_BYTES, TC_SLAB_BYTES, R.full(pq));
+    ++pq;
+  };
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(bar_full(i), 1); mbar_init(bar_peer(i), 1); mbar_init(bar_empty(i), 1); }
-    for (int t = 0; t < NT; ++t) { mbar_init(bar_tfull(t), 1); mbar_init(bar_aready(t), 8 * kPair); }
-    fence_mbar_init();
+    R.init();
+    for (int i = 0; i < TC_NSLOT; ++i) produce();
   }
-  if (threadIdx.x >= 64) {
-    const int e = threadIdx.x - 64;
-    s_walpha[e] = __ldg(P.w_alpha + e);
-  }
-  if (warp == 1) {
-    tmem_alloc<kPair>(smem_u32(tmem_ptr_smem), 512);
-    tmem_relinquish<kPair>();
-  }
-  tc_fence_before();
   __syncthreads();
-  if (kPair == 2) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  auto release = [&](uint32_t qq) {
+    if (wtid == 0) mbar_arrive_local(R.empty(qq));
+    if (threadIdx.x == 0) produce();
+    __syncwarp();
+  };
+  const float S = __ldg(P.scale);
 
-  const long long tiles_per_round = n_pairs * NT;
-  const long long n_rounds = (P.n_tiles + tiles_per_round - 1) / tiles_per_round;
-
-  if (warp == 0) {
-    // =============================== bulk-TMA producer ===============================
-    if (lane == 0) {
-      const uint8_t* img = P.wimg + (size_t)rank * P.image_bytes;
-      uint32_t q = 0;
-      for (long long round = 0; round < n_rounds; ++round)
-        for (int k = 0; k < BW_SLABS; ++k, ++q) {
-          const uint32_t slot = q % NSLOT, gen = q / NSLOT;
-          mbar_wait(bar_empty(slot), (gen & 1) ^ 1);
-          mbar_arrive_expect_tx(bar_full(slot), C::SLOT_BYTES);
-          bulk_g2s(sbase + C::OFF_RING + slot * C::SLOT_BYTES, img + (size_t)k * C::SLOT_BYTES, C::SLOT_BYTES, bar_full(slot));
-        }
-    }
-  } else if (warp == 1) {
-    if (rank == 0) {
-      // ======================= MMA issuer (leader CTA): whole warp, warp-uniform, one elected lane issues =======================
-      uint32_t issuer = 0;
-      asm volatile(
-          "{\n\t.reg .pred p;\n\t.reg .b32 r;\n\telect.sync r|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(issuer));
-      constexpr uint32_t idesc = make_idesc(128 * kPair, 256);
-      uint32_t q0 = 0, nstep = 0;
-      for (long long round = 0; round < n_rounds; ++round) {
-        for (int b = 0; b < BW_STEPS; ++b, ++nstep) {
-          const int nkb = bw_nkb(b);
-          for (int t = 0; t < NT; ++t) {
-            mbar_wait(bar_aready(t), nstep & 1);
-            tc_fence_after();
-            if (t == 0 && issuer) BW_TRACE(0, 0, nstep);
-            const uint32_t d_tmem = tmem_base + t * 256;
-            for (int kb = 0; kb < nkb; ++kb) {
-              const uint32_t q = q0 + kb, slot = q % NSLOT, gen = q / NSLOT;
-              if (t == 0) {
-                mbar_wait(bar_full(slot), gen & 1);
-                if (kPair == 2) mbar_wait(bar_peer(slot), gen & 1);
-                tc_fence_after();
-              }
-              const uint64_t a_desc = make_desc(sbase + C::OFF_ACT + (t * 4 + kb) * TC_KB_BYTES);
-              const uint64_t b_desc = make_desc(sbase + C::OFF_RING + slot * C::SLOT_BYTES);
-              if (issuer) {
-                umma_f16<kPair>(d_tmem, a_desc, b_desc, idesc, kb != 0);
-                umma_f16<kPair>(d_tmem, a_desc + 2, b_desc + 2, idesc, 1);
-                umma_f16<kPair>(d_tmem, a_desc + 4, b_desc + 4, idesc, 1);
-                umma_f16<kPair>(d_tmem, a_desc + 6, b_desc + 6, idesc, 1);
-                if (t == NT - 1) umma_commit<kPair>(bar_empty(slot));
-              }
-              __syncwarp();
-            }
-            if (issuer) {
-              umma_commit<kPair>(bar_tfull(t));
-              if (t == 0) BW_TRACE(0, 1, nstep);
-            }
-            __syncwarp();
-          }
-          q0 += nkb;
-        }
+  float d[128];
+  uint32_t qbase = 0;
+  for (long long it = 0; it < my_tiles; ++it) {
+    const long long row0 = (blockIdx.x + it * gridDim.x) * 128 + wg * TC_WG_ROWS;
+    const long long iA = row0 + rA, iB = iA + 8;
+    // ---- head: dVpre of row wtid / 2, channels 64 (wtid & 1) .. +63 = A k-block wtid & 1 ----
+    if (wtid == 0) tma_store_wait_read();           // the last step's gradient stores read the A buffer
+    wg_sync(wg);
+    {
+      const int r = wtid >> 1, h = wtid & 1;
+      const long long i = row0 + r;
+      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+      uint4 vm = make_uint4(0, 0, 0, 0);
+      if (i < P.n) {
+        g = __ldg(reinterpret_cast<const float4*>(P.d_raw) + i);
+        vm = __ldg(reinterpret_cast<const uint4*>(P.st_m + ((size_t)8 * P.n + i) * 8));
       }
-    } else {
-      // =============================== relay (peer CTA of a pair) ===============================
-      if (lane == 0) {
-        uint32_t q = 0;
-        for (long long round = 0; round < n_rounds; ++round)
-          for (int k = 0; k < BW_SLABS; ++k, ++q) {
-            const uint32_t slot = q % NSLOT, gen = q / NSLOT;
-            mbar_wait(bar_full(slot), gen & 1);
-            mbar_arrive_cluster(bar_peer(slot), 0);
-          }
-      }
-    }
-  } else {
-    // ========================= epilogue: 8 warps, both warpgroups drain every tile (column halves) =========================
-    const int ew = warp - 2;
-    const int g = ew >> 2;                         // column half; also: the tile whose head (dVpre row) this thread builds
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    uint32_t nstep = 0;
-    const float S = __ldg(P.scale);
-
-    auto publish = [&](int t) {
-      fence_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(bar_aready(t), 0);
-    };
-    auto sample_index = [&](long long round, int t) { return (((round * n_pairs + pair_id) * NT + t) * kPair + rank) * 128 + row; };
-    auto tile_valid = [&](long long round, int t) {
-      return ((round * n_pairs + pair_id) * NT + t) < P.n_tiles && sample_index(round, t) < P.n;
-    };
-    // head of tile g, round r: dVpre row (128 channels) in registers, computed one round ahead
-    uint32_t head[64];
-    // The head needs, per row, dL/d raw (16 B) and the 128 ReLU sign bits of the views layer (16 B): both are
-    // fetched a few steps before they are used (prefetch_head), so building the head is pure arithmetic.
-    float4 gr_next = make_float4(0.f, 0.f, 0.f, 0.f);
-    uint4 vm_next = make_uint4(0, 0, 0, 0);
-    auto prefetch_head = [&](long long round) {
-      gr_next = make_float4(0.f, 0.f, 0.f, 0.f);
-      vm_next = make_uint4(0, 0, 0, 0);
-      if (tile_valid(round, g)) {
-        const long long i = sample_index(round, g);
-        gr_next = __ldg(reinterpret_cast<const float4*>(P.d_raw) + i);
-        vm_next = __ldg(reinterpret_cast<const uint4*>(P.st_m + ((size_t)8 * P.n + i) * 8));
-      }
-    };
-    auto build_head = [&]() {
-      const float gx = gr_next.x * S, gy = gr_next.y * S, gz = gr_next.z * S;
-      const uint32_t vw[4] = {vm_next.x, vm_next.y, vm_next.z, vm_next.w};
+      const float gx = g.x * S, gy = g.y * S, gz = g.z * S;
+      const uint32_t vw[4] = {vm.x, vm.y, vm.z, vm.w};
+      uint32_t head[32];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        // columns 8j .. 8j+7 live in word j/4, 16-bit half (j/2)%2; pair p of that group: bit p = even column, bit 8+p = odd
+      for (int jj = 0; jj < 8; ++jj) {
+        const int j = 8 * h + jj;                   // columns 8j .. 8j+7: word j/4, 16-bit half (j/2)%2
         const uint32_t bits16 = vw[j >> 2] >> (16 * ((j >> 1) & 1));
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const int c = 8 * j + 2 * k, pr = 4 * (j & 1) + k;
-          float x0 = fmaf(gx, c_bw_wrgb[c], fmaf(gy, c_bw_wrgb[128 + c], gz * c_bw_wrgb[256 + c]));
-          float x1 = fmaf(gx, c_bw_wrgb[c + 1], fmaf(gy, c_bw_wrgb[129 + c], gz * c_bw_wrgb[257 + c]));
+          float x0 = fmaf(gx, s_wrgb[c], fmaf(gy, s_wrgb[128 + c], gz * s_wrgb[256 + c]));
+          float x1 = fmaf(gx, s_wrgb[c + 1], fmaf(gy, s_wrgb[129 + c], gz * s_wrgb[257 + c]));
           if (!((bits16 >> pr) & 1u)) x0 = 0.f;
           if (!((bits16 >> (8 + pr)) & 1u)) x1 = 0.f;
-          head[4 * j + k] = pack_f16x2(x0, x1, false);
+          head[4 * jj + k] = pack_f16x2(x0, x1, false);
         }
       }
-    };
-    auto store_head = [&](int t) {                  // 128 channels -> A k-blocks 0 and 1 of tile t
-      uint8_t* act = smem + C::OFF_ACT + t * 4 * TC_KB_BYTES;
 #pragma unroll
-      for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<uint4*>(act + kb * TC_KB_BYTES + row * 128 + ((j ^ (row & 7)) << 4)) =
-              make_uint4(head[32 * kb + 4 * j], head[32 * kb + 4 * j + 1], head[32 * kb + 4 * j + 2], head[32 * kb + 4 * j + 3]);
-    };
-    auto load_mask = [&](long long round, int t, int plane) {
-      if (!tile_valid(round, t)) return make_uint4(0, 0, 0, 0);
-      return __ldg(reinterpret_cast<const uint4*>(P.st_m + ((size_t)plane * P.n + sample_index(round, t)) * 8) + (g ^ t));
-    };
-    if (n_rounds > 0) { prefetch_head(0); build_head(); }
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<uint4*>(act + h * TC_KB_BYTES + r * 128 + ((j ^ (r & 7)) << 4)) =
+            make_uint4(head[4 * j], head[4 * j + 1], head[4 * j + 2], head[4 * j + 3]);
+    }
+    fence_async_smem();
+    wg_sync(wg);
+    if (wtid == 0) tma_store_rows(&P.map_v, abase, 0, 2, row0, 0);   // dL/d(views pre-activation)
+    const float daA = iA < P.n ? S * __ldg(P.d_raw + 4 * iA + 3) : 0.f;
+    const float daB = iB < P.n ? S * __ldg(P.d_raw + 4 * iB + 3) : 0.f;
 
-    // Column ownership: for tile t this thread drains columns [(g ^ t) * 128, +128) = A k-blocks 2(g^t), 2(g^t)+1 of its
-    // row in every step.  The warpgroup that builds the head of tile t (g == t) is therefore the one that owns k-blocks
-    // 0 and 1 of that tile, and every write / TMA read of a slice of the A buffer is ordered inside one warp.
-    for (long long round = 0; round < n_rounds; ++round) {
-      float da[NT];
-      uint4 mnext[NT];
-#pragma unroll
-      for (int t = 0; t < NT; ++t) {
-        if (g == t) {
-          // the last step of the previous round stored this slice by TMA: it must have been read
-          if (lane == 0) tma_store_wait_read<0>();
-          __syncwarp();
-          store_head(t);
-          fence_async_smem();
-          __syncwarp();
-          const long long i0 = sample_index(round, t) - lane;
-          if (lane == 0 && i0 < P.n) {                  // dL/d(views pre-activation) leaves from the A buffer as well
-            const uint32_t src = sbase + C::OFF_ACT + t * 4 * TC_KB_BYTES + quad * 32 * 128;
-            tma_store_3d(&P.map_v, src, 0, (int)i0, 0);
-            tma_store_3d(&P.map_v, src + TC_KB_BYTES, 64, (int)i0, 0);
-            tma_store_commit();
-          }
-        }
-        publish(t);
-        da[t] = tile_valid(round, t) ? S * __ldg(P.d_raw + 4 * sample_index(round, t) + 3) : 0.f;
-        mnext[t] = load_mask(round, t, 7);          // step b1 masks with [X8 > 0] = plane 7
+    for (int b = 0; b < BW_STEPS; ++b) {
+      const int nkb = bw_nkb(b);
+      // masks of this step (plane 8 - b), fetched while the MMAs run
+      uint32_t mA[8], mB[8];
+      if (b >= 1) {
+        const uint32_t* m = P.st_m + (size_t)(8 - b) * P.n * 8;
+        load_signs(m, iA, P.n, mA);
+        load_signs(m, iB, P.n, mB);
       }
-      for (int b = 0; b < BW_STEPS; ++b, ++nstep) {
-        uint4 mcur[NT];
+      wgmma_fence();
+      for (int kb = 0; kb < nkb; ++kb) {
+        const uint32_t qq = qbase + kb;
+        R.wait_full(qq);
+        const uint64_t a_desc = gmma_desc_k(abase + kb * TC_KB_BYTES), b_desc = gmma_desc_k(R.slot(qq));
 #pragma unroll
-        for (int t = 0; t < NT; ++t) mcur[t] = mnext[t];
-        if (b >= 1 && b < BW_STEPS - 1) {           // masks of step b+1: plane 8-(b+1), one full step ahead
-#pragma unroll
-          for (int t = 0; t < NT; ++t) mnext[t] = load_mask(round, t, 7 - b);
-        }
-#pragma unroll
-        for (int t = 0; t < NT; ++t) {
-          uint8_t* act = smem + C::OFF_ACT + t * 4 * TC_KB_BYTES;
-          const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16) + t * 256;
-          const int gc = g ^ t;                       // column half of this thread for tile t
-          mbar_wait(bar_tfull(t), nstep & 1);
-          tc_fence_after();
-          if (t == 0 && ew == 0 && lane == 0) BW_TRACE(1, 0, nstep);
-          // this warp's slice is the source of the TMA store it issued one step ago (the other tile's may still
-          // fly); in step 0 the head's store of this round may be the most recent one: wait for everything
-          if (lane == 0) { if (b == 0) tma_store_wait_read<0>(); else tma_store_wait_read<1>(); }
-          __syncwarp();
-          if (b == 0) bw_step<false, false>(t_lane, gc * 128, 0.f, s_walpha, mcur[t], act, row);
-          else if (b == 1) bw_step<true, true>(t_lane, gc * 128, da[t], s_walpha, mcur[t], act, row);
-          else bw_step<false, true>(t_lane, gc * 128, 0.f, s_walpha, mcur[t], act, row);
-          if (t == 0 && ew == 0 && lane == 0) BW_TRACE(1, 1, nstep);
-          const long long i0 = sample_index(round, t) - lane;              // first row of this warp
-          const bool issue = lane == 0 && i0 < P.n;
-          const uint32_t src = sbase + C::OFF_ACT + (t * 4 + 2 * gc) * TC_KB_BYTES + quad * 32 * 128;
-          const CUtensorMap* m = b == 0 ? &P.map_f : &P.map_pre;
-          const int plane = b == 0 ? 0 : 8 - b;
-          if (b < BW_STEPS - 1) {
-            publish(t);                               // the MMA thread first: the store and the next MMAs only read
-          } else {
-            fence_async_smem();                       // last step: nothing to hand over, only the store
-            tc_fence_before();
-            __syncwarp();
-          }
-          if (issue) {
-            tma_store_3d(m, src, 128 * gc, (int)i0, plane);
-            tma_store_3d(m, src + TC_KB_BYTES, 128 * gc + 64, (int)i0, plane);
-            tma_store_commit();
-          }
-          if (t == 0 && ew == 0 && lane == 0) BW_TRACE(1, 2, nstep);
-        }
-        if (b == 1 && round + 1 < n_rounds) prefetch_head(round + 1);
-        if (b == 4 && round + 1 < n_rounds) build_head();
+        for (int k = 0; k < 4; ++k) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+        wgmma_commit();
+        if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      release(qbase + nkb - 1);
+      qbase += nkb;
+      if (wtid == 0) tma_store_wait_read();
+      wg_sync(wg);
+      if (b == 0) bw_epi<false, false>(d, act, rA, q, s_walpha, 0.f, 0.f, mA, mB);
+      else if (b == 1) bw_epi<true, true>(d, act, rA, q, s_walpha, daA, daB, mA, mB);
+      else bw_epi<false, true>(d, act, rA, q, s_walpha, 0.f, 0.f, mA, mB);
+      fence_async_smem();
+      wg_sync(wg);
+      if (wtid == 0) {
+        if (b == 0) tma_store_rows(&P.map_f, abase, 0, 4, row0, 0);
+        else tma_store_rows(&P.map_pre, abase, 0, 4, row0, 8 - b);
       }
     }
   }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (kPair == 2) cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<kPair>(tmem_base, 512);
-  }
+  if (wtid == 0) tma_store_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -392,23 +218,20 @@ __device__ __forceinline__ float bw_src_weight(const BwPackSrc& S, int b, int n,
   return S.wt[l][(size_t)((l == 5 ? NM_POS_PE : 0) + n) * 256 + out];           // layer 5 input = [PE(63), hidden]
 }
 
-__global__ void k_bw_pack(BwPackSrc S, int kpair, uint32_t image_bytes, __half* __restrict__ out, const float* __restrict__ rgb_t,
+__global__ void k_bw_pack(BwPackSrc S, uint32_t image_bytes, __half* __restrict__ out, const float* __restrict__ rgb_t,
                           float* __restrict__ wrgb) {
-  const int rank = blockIdx.y;
   const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (rank == 0 && e < 384) wrgb[e] = rgb_t[(e & 127) * 3 + (e >> 7)];      // [128][3] (api.cu layout) -> [3][128]
+  if (e < 384) wrgb[e] = rgb_t[(e & 127) * 3 + (e >> 7)];      // [128][3] (api.cu layout) -> [3][128]
   if (e * 2 >= image_bytes) return;
-  const uint32_t slot_bytes = 32768u / kpair;
   const uint32_t byte = (uint32_t)(e * 2);
-  const int k = byte / slot_bytes;                     // slab index
+  const int k = byte / TC_SLAB_BYTES;                  // slab index
   const int b = k < 2 ? 0 : 1 + (k - 2) / 4;
   const int kb = k < 2 ? k : (k - 2) % 4;
-  const uint32_t in_slab = byte - k * slot_bytes;
-  const int n_local = in_slab >> 7;
-  const int chunk = ((in_slab & 127) >> 4) ^ (n_local & 7);
+  const uint32_t in_slab = byte - k * TC_SLAB_BYTES;
+  const int n = in_slab >> 7;
+  const int chunk = ((in_slab & 127) >> 4) ^ (n & 7);
   const int kk = chunk * 8 + ((in_slab & 15) >> 1);
-  const int n = rank * (256 / kpair) + n_local;
-  out[(size_t)rank * (image_bytes / 2) + e] = __float2half_rn(bw_src_weight(S, b, n, kb, kk));
+  out[e] = __float2half_rn(bw_src_weight(S, b, n, kb, kk));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -490,76 +313,41 @@ int nm_impl_pe_backward(nm_ctx* ctx, const NmNet& net, int which, const float* x
   return NM_OK;
 }
 
-static int bw_pair_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("NEUMAN_TC_PAIR");
-    mode = (e && e[0] == '1') ? 1 : 2;
-  }
-  return mode;
-}
-
 int nm_tc_pack_bwd(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
-  const int kpair = bw_pair_mode();
-  const uint32_t image_bytes = (uint32_t)BW_SLABS * (32768u / kpair);
-  const size_t halfs = (size_t)kpair * image_bytes / 2;
-  if (!net.f16_bwd) NM_CHECK_CUDA(ctx, cudaMalloc(&net.f16_bwd, halfs * sizeof(__half)));
+  const uint32_t image_bytes = (uint32_t)BW_SLABS * TC_SLAB_BYTES;
+  if (!net.f16_bwd) NM_CHECK_CUDA(ctx, cudaMalloc(&net.f16_bwd, image_bytes));
   if (!net.bw_wrgb) NM_CHECK_CUDA(ctx, cudaMalloc(&net.bw_wrgb, 384 * sizeof(float)));
   BwPackSrc S;
   for (int l = 0; l < 8; ++l) S.wt[l] = net.f32 + net.o_pts_w[l];
   S.feat_t = net.f32 + net.o_feat_w; S.views_t = net.f32 + net.o_views_w;
-  dim3 grid((unsigned)((image_bytes / 2 + 255) / 256), kpair);
-  k_bw_pack<<<grid, 256, 0, st>>>(S, kpair, image_bytes, net.f16_bwd, net.f32 + net.o_rgb_w, net.bw_wrgb);
+  k_bw_pack<<<(unsigned)((image_bytes / 2 + 255) / 256), 256, 0, st>>>(S, image_bytes, net.f16_bwd, net.f32 + net.o_rgb_w, net.bw_wrgb);
   NM_CHECK_LAUNCH(ctx);
   net.bwd_packed = true;
   return NM_OK;
 }
 
-template <int kPair>
-static int launch_bwd(nm_ctx* ctx, const BwParams& P, cudaStream_t st) {
-  using C = BwCfg<kPair>;
-  NM_SET_SMEM_ONCE(ctx, (k_mlp_tc_bwd<kPair>), C::SMEM_BYTES);
-  int ctas = ctx->sm_count - (ctx->sm_count % kPair);
-  long long need = (P.n_tiles * kPair + C::NT - 1) / C::NT;
-  if (need < ctas) ctas = (int)((need + kPair - 1) / kPair * kPair);
-  if (ctas < kPair) ctas = kPair;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(ctas);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kPair; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NM_CHECK_CUDA(ctx, cudaLaunchKernelEx(&cfg, k_mlp_tc_bwd<kPair>, P));
-  NM_LAUNCHED(ctx);
-  return NM_OK;
-}
-
 int nm_tc_backward(nm_ctx* ctx, NmNet& net, const float* d_raw, const float* scale, int64_t n, const __half* st_v,
                    const uint32_t* st_m, __half* g_pre, __half* g_f, __half* g_v, cudaStream_t st) {
-  const int kpair = bw_pair_mode();
   if (!net.bwd_packed) {
     int rc = nm_tc_pack_bwd(ctx, net, st);
     if (rc != NM_OK) return rc;
   }
   BwParams P;
   P.wimg = reinterpret_cast<const uint8_t*>(net.f16_bwd);
-  P.image_bytes = (uint32_t)BW_SLABS * (32768u / kpair);
   P.d_raw = d_raw; P.scale = scale;
   P.w_alpha = net.f32 + net.o_alpha_w;
-  NM_CHECK_CUDA(ctx, cudaMemcpyToSymbolAsync(c_bw_wrgb, net.bw_wrgb, 384 * sizeof(float), 0, cudaMemcpyDeviceToDevice, st));
+  P.w_rgb = net.bw_wrgb;
   P.st_m = st_m;
-  P.g_pre = g_pre; P.g_f = g_f; P.g_v = g_v;
   P.n = n;
-  P.n_tiles = (n + 128 * kpair - 1) / (128 * kpair);
-  P.trace = nullptr;
-  if (const char* e = getenv("NEUMAN_TC_TRACE_BWD")) P.trace = reinterpret_cast<long long*>(strtoull(e, nullptr, 0));
+  P.n_tiles = (n + 127) / 128;
   if (n >= (int64_t)0x7fff0000) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_backward: n too large for one call");
   if (tc_make_store_map(&P.map_pre, g_pre, 8, (uint64_t)n, 256) || tc_make_store_map(&P.map_f, g_f, 1, (uint64_t)n, 256) ||
       tc_make_store_map(&P.map_v, g_v, 1, (uint64_t)n, 128))
     NM_FAIL(ctx, NM_ERR_CUDA, "nm_mlp_backward: cuTensorMapEncodeTiled failed");
-  return kpair == 2 ? launch_bwd<2>(ctx, P, st) : launch_bwd<1>(ctx, P, st);
+  NM_SET_SMEM_ONCE(ctx, k_mlp_tc_bwd, BwCfg::SMEM_BYTES);
+  long long ctas = ctx->sm_count;
+  if (P.n_tiles < ctas) ctas = P.n_tiles > 0 ? P.n_tiles : 1;
+  k_mlp_tc_bwd<<<(unsigned)ctas, BwCfg::THREADS, BwCfg::SMEM_BYTES, st>>>(P);
+  NM_CHECK_LAUNCH(ctx);
+  return NM_OK;
 }

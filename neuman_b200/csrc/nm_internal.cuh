@@ -31,9 +31,7 @@ struct NmNet {
   // tensor-core layout (see mlp_tc.cu for the tile format)
   __half* f16 = nullptr;
   size_t f16_halfs = 0;
-  float* tc_bias = nullptr;         // epilogue constants: 10 bias rows, alpha weights, output biases (mlp_tc.cu TcParams::consts)
-  float* consts_host = nullptr;     // pinned host copy (kernel parameters of the inference launches), refreshed lazily
-  bool consts_host_valid = false;
+  float* tc_bias = nullptr;         // epilogue constants: alpha weights, output biases (mlp_tc.cu k_tc_consts)
   __half* f16_bwd = nullptr;        // transposed slabs for the backward chain (mlp_tc_bwd.cu), packed on first use
   float* bw_wrgb = nullptr;         // rgb_linear.weight as [3][128] for the backward kernel's constant bank
   bool bwd_packed = false;
@@ -72,7 +70,7 @@ struct NmMesh {
 
 struct nm_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   std::string err;
   int64_t launches = 0;
   NmNet nets[NM_MAX_NET_SLOTS];

@@ -1,12 +1,14 @@
-// tcgen05 / TMA / mbarrier PTX wrappers and UMMA descriptors shared by the tensor-core MLP kernels
-// (mlp_tc.cu: inference + training forward, mlp_tc_bwd.cu: backward chain).
+// wgmma / bulk-TMA / mbarrier PTX wrappers and GMMA shared-memory descriptors shared by the tensor-core kernels
+// (mlp_tc.cu: inference + training forward, mlp_tc_bwd.cu: backward chain, dw_gemm.cu: weight gradients).
 #pragma once
 #include "nm_internal.cuh"
 
 #define TC_STEPS 11
-#define TC_CONST_FLOATS 272         // epilogue constants of the forward kernel (mlp_tc.cu: TcParams::consts)
-#define TC_KB_BYTES 16384          // one A k-block: 128 rows x 128 B
-#define TC_BIAS_STRIDE 256
+#define TC_CONST_FLOATS 272         // epilogue constants of the forward kernel (mlp_tc.cu: k_tc_consts)
+#define TC_WG_ROWS 64              // sample rows per consumer warpgroup (wgmma M = 64)
+#define TC_KB_BYTES (TC_WG_ROWS * 128)   // one A k-block of a warpgroup: 64 rows x 128 B
+#define TC_SLAB_BYTES 32768        // one weight k-block: 256 rows x 128 B
+#define TC_NSLOT 4                 // depth of the weight ring
 
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -27,29 +29,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "DONE:\n\t"
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
-// polling wait with a sleep between probes: for roles that run far ahead of their consumer (the bulk-TMA
-// producer, the relay, the encoding warps), so that their spinning does not burn issue slots and power
-__device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity, uint32_t ns) {
-  uint32_t done = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) break;
-    __nanosleep(ns);
-  }
-}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// arrive on the barrier at the same offset in CTA `rank` of the cluster (works for rank == self)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(bar), "r"(rank) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_local(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -60,101 +41,80 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+// barrier of the 128 threads of one warpgroup (ids 1.. : 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
+
+// GMMA shared-memory descriptors, SWIZZLE_128B (layout type 1 at bits [62,64)), base offset 0 (1024-byte aligned atoms):
+// start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46)
+// K-major: rows of 128 B (64 fp16 of K), 8-row atoms 1024 B apart; the K = 16 slices of an atom start 32 B apart
+__device__ __forceinline__ uint64_t gmma_desc_k(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// MN-major: rows = K of 128 B (64 fp16 of M or N), 8-row K groups 1024 B apart, 64-wide M/N atoms `lbo` bytes apart
+__device__ __forceinline__ uint64_t gmma_desc_mn(uint32_t saddr, uint32_t lbo) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
 }
 
-template <int kPair>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  if (kPair == 2)
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-  else
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-}
-template <int kPair>
-__device__ __forceinline__ void tmem_relinquish() {
-  if (kPair == 2) asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  else asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kPair>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  if (kPair == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-  else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads / writes of accumulator registers across wgmma issue / wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16 operands, fp32 accumulate
-template <int kPair>
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-  if (kPair == 2) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum) : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum) : "memory");
-  }
-}
-// arrive::one on `bar` (same offset in every CTA of the pair) once all prior MMAs of this thread retire
-template <int kPair>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if (kPair == 2) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"((uint16_t)3) : "memory");
-  } else {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-  }
-}
-
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row atoms 1024 B apart
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout=2 [61,64))
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-// K-major operand WITHOUT swizzle: core matrices of 8 rows x 16 bytes (rows contiguous), `lbo` bytes between the two core
-// matrices of a K = 16 step, `sbo` bytes between 8-row groups (0: every group reads the same core matrices)
-__device__ __forceinline__ uint64_t make_desc_ns(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | ((uint64_t)1 << 46);
-}
-// UMMA instruction descriptor, kind::f16: D=f32 (bit4), A=B=f16 (0), both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 operands from shared memory, fp32 accumulators in registers of the
+// warpgroup: thread (warp w, lane l) holds rows 16w + l/4 (+8) and columns 8j + 2(l%4) (+1) as d[4j + {0,1,2,3}].
+// `accum` = 0 overwrites D.  The _mn variants read both operands MN-major.
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accum) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(accum));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_n128(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accum) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accum));
 }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t (&v)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(taddr));
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(accum));
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_n256_mn(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_n16_mn(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(accum));
+}
 
 // {lo, hi} -> packed f16x2 (lo in the low half), optional ReLU
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi, bool relu) {
@@ -164,16 +124,21 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi, bool relu) {
   return d;
 }
 
+// byte offset of the 4-byte pair (row, columns c, c+1; c even) inside a K-major SWIZZLE_128B block of 64 columns
+__device__ __forceinline__ uint32_t swz_off(int row, int c) {
+  return row * 128 + ((((c & 63) >> 3) ^ (row & 7)) << 4) + ((c & 7) << 1);
+}
 
 // ---------------------------------------------------------------------------------------------
-// TMA tensor stores (shared -> global) of activation blocks.  The UMMA SWIZZLE_128B K-major block layout is the
-// TMA SWIZZLE_128B box layout, so a warp's 32 rows x 64 columns of an activation k-block (4 KB, contiguous in
-// shared memory) go out as one box and land row-major in the HBM plane.
+// TMA tensor stores (shared -> global) of activation blocks.  The GMMA SWIZZLE_128B K-major block layout is the
+// TMA SWIZZLE_128B box layout, so 32 rows x 64 columns of an activation k-block (4 KB, contiguous in shared memory)
+// go out as one box and land row-major in the HBM plane.
 // ---------------------------------------------------------------------------------------------
 #include <cuda.h>
 
-// [planes][rows][width] fp16, box = 64 columns x 32 rows x 1 plane
-inline int tc_make_store_map(CUtensorMap* map, const void* base, uint64_t planes, uint64_t rows, uint32_t width) {
+// [planes][rows][width] fp16, box = 64 columns x box_rows rows x 1 plane
+inline int tc_make_map(CUtensorMap* map, const void* base, uint64_t planes, uint64_t rows, uint32_t width, uint32_t box_rows,
+                       CUtensorMapL2promotion l2) {
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -186,12 +151,14 @@ inline int tc_make_store_map(CUtensorMap* map, const void* base, uint64_t planes
   }
   const cuuint64_t dims[3] = {width, rows, planes};
   const cuuint64_t strides[2] = {(cuuint64_t)width * 2, (cuuint64_t)rows * width * 2};
-  const cuuint32_t box[3] = {64, 32, 1};
+  const cuuint32_t box[3] = {64, box_rows, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+inline int tc_make_store_map(CUtensorMap* map, const void* base, uint64_t planes, uint64_t rows, uint32_t width) {
+  return tc_make_map(map, base, planes, rows, width, 32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t smem_src, int col, int row, int plane) {
@@ -199,6 +166,31 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t sm
                "r"(col), "r"(row), "r"(plane) : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// the issuing thread waits until at most N of its committed store groups still read shared memory
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// the issuing thread waits until none of its committed store groups still reads shared memory
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... or until all of them have completed (before the kernel exits)
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// A warpgroup's 64 rows x (kb1 - kb0) k-blocks of an activation buffer -> rows [row0, row0 + 64) of `plane`, columns
+// 64 kb0 .. 64 kb1 (rows past the end of the plane are clipped by the TMA unit).  One thread issues.
+__device__ __forceinline__ void tma_store_rows(const CUtensorMap* map, uint32_t act, int kb0, int kb1, long long row0, int plane) {
+  for (int kb = kb0; kb < kb1; ++kb)
+    for (int h = 0; h < 2; ++h)
+      tma_store_3d(map, act + kb * TC_KB_BYTES + h * 32 * 128, 64 * kb, (int)(row0 + 32 * h), plane);
+  tma_store_commit();
+}
+
+// One warpgroup's view of the weight ring: the slabs of a launch are consumed in a fixed order by both warpgroups; a slab's
+// slot is refilled once both have released it.  Thread 0 of the CTA is the producer: it issues the first TC_NSLOT slabs
+// and, after each of its own releases, the slab TC_NSLOT places further on.
+struct TcRing {
+  uint32_t ring, bar;       // shared addresses: TC_NSLOT slots of TC_SLAB_BYTES; full[TC_NSLOT] then empty[TC_NSLOT]
+  __device__ uint32_t slot(uint32_t q) const { return ring + (q % TC_NSLOT) * TC_SLAB_BYTES; }
+  __device__ uint32_t full(uint32_t q) const { return bar + 8 * (q % TC_NSLOT); }
+  __device__ uint32_t empty(uint32_t q) const { return bar + 8 * (TC_NSLOT + q % TC_NSLOT); }
+  __device__ void wait_full(uint32_t q) const { mbar_wait(full(q), (q / TC_NSLOT) & 1); }
+  __device__ void init() const {
+    for (int i = 0; i < TC_NSLOT; ++i) { mbar_init(bar + 8 * i, 1); mbar_init(bar + 8 * (TC_NSLOT + i), 2); }
+    fence_mbar_init();
+  }
+};

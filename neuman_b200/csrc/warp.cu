@@ -507,7 +507,7 @@ extern "C" int nm_warp_to_canonical(nm_ctx* ctx, int actor, const float* pts, in
   }
   {
     static const int lg_env = [] { const char* e = getenv("NEUMAN_WARP_PACKET"); return e ? atoi(e) : -1; }();
-    int lg = (lg_env >= 0 && lg_env <= 3) ? lg_env : 1;   // default: 2 rays x 16 samples (profiles/r02_configs.md)
+    int lg = (lg_env >= 0 && lg_env <= 3) ? lg_env : 1;   // default: 2 rays x 16 samples
     while (lg > 0 && (S % (32 >> lg) != 0 || R < (1 << lg))) --lg;
     long long warps = lg == 0 ? (n + 31) / 32 : ((R + (1 << lg) - 1) >> lg) * (long long)(S / (32 >> lg));
     k_warp_nearest<<<(unsigned)((warps + 3) / 4), 128, 0, st>>>(B, pts, (long long)R, (int)S, lg, fid);

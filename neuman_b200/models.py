@@ -163,7 +163,7 @@ class OffsetNet(nn.Module):
       * `output_linear` (3 x 256, any sign) is carried through the Joiner's non-negative head as y = relu(y) - relu(-y):
         feature rows 0..2 = +W_o, 3..5 = -W_o, a unit views layer, rgb = [I, -I].
     `forward_at_time` builds those weights with differentiable torch indexing (a few 256-wide tensors), runs the SAME
-    tcgen05 training / inference kernels as every other network (k_mlp_tc, k_mlp_tc_bwd, k_dw_gemm), and autograd carries
+    wgmma training / inference kernels as every other network (k_mlp_tc, k_mlp_tc_bwd, k_dw_gemm), and autograd carries
     the Joiner-shaped gradients back to this module's parameters.  `forward` uses it when the time column is constant and
     the architecture is the reference's default (8 x 256, skip 4, 10 log-spaced frequencies); otherwise it evaluates the
     network with library GEMMs (torch.nn.functional.linear, float32), which is also the CPU path."""

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY (oracle) -- float64 restatement of the three libigl calls on the NeuMan
 hot path.  **Parity unpinned**: libigl 2.2.1 (environment.yml:13) is a third-party C++ dependency
-that is absent from /root/reference and from this image, and the reference holds no golden vectors
+that is not part of the reference tree, and the reference holds no golden vectors
 at this boundary (SURVEY.md §8c).  This file restates the *published* semantics of
 
   igl.point_mesh_squared_distance(P, V, F) -> (sqrD, I, C)   call site utils/ray_utils.py:53

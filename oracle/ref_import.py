@@ -1,40 +1,25 @@
-"""TEST INFRASTRUCTURE ONLY -- imports the *unmodified* reference (apple/ml-neuman) from
-/root/reference so that the oracle restatement (oracle/neuman_oracle.py) can be validated against
-it and golden vectors can be generated (tools/make_golden.py).
+"""TEST INFRASTRUCTURE ONLY -- imports the *unmodified* reference (apple/ml-neuman) from the tree named by
+$NEUMAN_REFERENCE, so that golden vectors can be generated from it (tools/make_golden*.py).  Nothing in the test suite,
+bench.py or the library needs it.
 
-The reference imports eight third-party packages that are absent in this image and are NOT used on
-the hot path (SURVEY.md §8c): igl, pytorch3d, open3d, matplotlib, imageio, lpips, tensorboardX,
-skimage.  They are replaced by empty stub modules.  `igl` is special: three of its functions ARE on
-the hot path (utils/ray_utils.py:53,55,70); the stub routes them to the float64 brute-force
-restatement in oracle/mesh_oracle.py ("parity unpinned" for that one stage -- libigl 2.2.1 itself
-is not available, environment.yml:13).
-
-/root/reference does not exist on the GPU box; there only the unmodified copy under baseline/_ref (git-ignored,
-tools/install_reference.py) can be imported, by bench.py's CPU arm and tests/test_gpu_dropin.py.
+The reference imports eight third-party packages that are NOT used on the hot path (SURVEY.md §8c): igl, pytorch3d,
+open3d, matplotlib, imageio, lpips, tensorboardX, skimage.  They are replaced by empty stub modules.  `igl` is special:
+three of its functions ARE on the hot path (utils/ray_utils.py:53,55,70); the stub routes them to the float64
+brute-force restatement in oracle/mesh_oracle.py ("parity unpinned" for that one stage -- libigl 2.2.1 itself is not
+available, environment.yml:13).
 """
 import importlib
 import os
 import sys
 import types
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 
 
-def _find_root():
-    """The reference tree: $NEUMAN_REFERENCE, else /root/reference (build container), else the unmodified copy that
-    tools/install_reference.py placed under baseline/_ref (it travels to the GPU box; used there by bench.py's CPU arm and
-    tests/test_gpu_dropin.py only)."""
-    for c in (os.environ.get("NEUMAN_REFERENCE"), "/root/reference", os.path.join(os.path.dirname(_HERE), "baseline", "_ref")):
-        if c and os.path.isdir(os.path.join(c, "utils")):
-            return c
-    return "/root/reference"
-
-
-REF_ROOT = _find_root()
+REF_ROOT = os.environ.get("NEUMAN_REFERENCE", "")
 
 
 def available():
-    return os.path.isdir(os.path.join(REF_ROOT, "utils"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "utils"))
 
 
 class _Anything:
@@ -92,7 +77,7 @@ def install_stubs():
 def load():
     """Returns a namespace with the reference's hot-path modules imported."""
     if not available():
-        raise RuntimeError(f"reference tree not found at {REF_ROOT}")
+        raise RuntimeError(f"reference tree not found (set NEUMAN_REFERENCE): {REF_ROOT!r}")
     install_stubs()
     if REF_ROOT not in sys.path:
         sys.path.insert(0, REF_ROOT)

@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
-    config.addinivalue_line("markers", "reference: needs the read-only reference tree at /root/reference")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
+    config.addinivalue_line("markers", "reference: needs the original project's tree, named by $NEUMAN_REFERENCE")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -25,4 +25,4 @@ def pytest_collection_modifyitems(config, items):
         if "gpu" in item.keywords and not has_gpu:
             item.add_marker(pytest.mark.skip(reason="no CUDA device"))
         if "reference" in item.keywords and not has_ref:
-            item.add_marker(pytest.mark.skip(reason="reference tree not present (GPU box)"))
+            item.add_marker(pytest.mark.skip(reason="reference tree not present ($NEUMAN_REFERENCE)"))

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY -- builds (g++) and binds (ctypes) the host emulation of the human-trainer kernels: the same
-kernel bodies as libneuman_b200.so compiles for sm_100a (neuman_b200/csrc/human_train_kernels.cuh,
+kernel bodies as libneuman_b200.so compiles for sm_90a (neuman_b200/csrc/human_train_kernels.cuh,
 smpl_train_kernels.cuh), executed serially on numpy arrays.  See cuda_emu.h."""
 import ctypes as C
 import os

@@ -31,7 +31,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, s), f"{s} declared in include/neuman_b200.h but not exported"
     # and the ctypes binding covers exactly the header
     assert sorted(_lib.SIGNATURES) == header_symbols()
-    assert b"sm_100a" in _lib.load().nm_version()
+    assert b"sm_90a" in _lib.load().nm_version()
 
 
 def test_no_gpu_fails_loudly():

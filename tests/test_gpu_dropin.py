@@ -1,8 +1,8 @@
-"""The drop-in under the reference's OWN callers on the B200 (SURVEY.md §8b): the unmodified reference (its copy under
-baseline/_ref, tools/install_reference.py) builds the networks, the captures and the HumanNeRF container, `neuman_b200.install()`
-rebinds its hot-path functions, and the reference's `render_*` / sampler / `Joiner.forward` entry points are then called
-exactly as `render_360.py`, `render_test_views.py`, `render_gathering.py` and the trainers' validation call them -- with
-CUDA modules and tensors.  Results are compared with the goldens the same reference produced on the CPU."""
+"""The drop-in on the GPU (SURVEY.md §8b): `neuman_b200.install()` rebinds the hot-path functions of modules with the
+reference's names and signatures (tests/standin_reference.py: the reference tree itself is not needed), and the `render_*` /
+sampler / `Joiner.forward` entry points are then called as `render_360.py`, `render_test_views.py`, `render_gathering.py`
+and the trainers' validation call them -- with CUDA modules and tensors.  Results are compared with the goldens the
+reference produced on the CPU."""
 import contextlib
 import io
 
@@ -13,8 +13,9 @@ import torch
 import neuman_b200 as nb
 from neuman_b200._lib import Context
 from oracle import neuman_oracle as no
-from oracle import ref_import, ref_opts, scenes
+from oracle import scenes
 from tests import util
+from tests.standin_reference import standin
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
@@ -22,22 +23,14 @@ TOL = 1e-4
 
 @pytest.fixture(scope="module")
 def ref():
-    if not ref_import.available():
-        pytest.skip("no reference copy (baseline/_ref is installed by tools/install_reference.py in the build container)")
-    r = ref_import.load()
-    r.mods = nb.install(ref_import.REF_ROOT)
-    assert nb.install(ref_import.REF_ROOT)["render_utils"] is r.mods["render_utils"]       # idempotent
-    yield r
-    from neuman_b200 import dropin
-    dropin.uninstall()
+    with standin() as r:
+        r.mods = nb.install()
+        assert nb.install()["render_utils"] is r.mods["render_utils"]       # idempotent
+        yield r
 
 
 def cap_of(ref, K, c2w, H, W, near=0.0, far=3.14):
-    cam = ref.pinhole_camera.PinholeCamera(W, H, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
-    pose = ref.camera_pose.CameraPose.from_camera_to_world(np.asarray(c2w).astype(np.float64))
-    cap = ref.captures.BasePinholeCapture(cam, pose)
-    cap.near, cap.far = {"bkg": near}, {"bkg": far}
-    return cap
+    return nb.SimpleCapture(np.asarray(K), np.asarray(c2w).astype(np.float64), H, W, near, far)
 
 
 def quiet(fn, *a, **k):
@@ -51,7 +44,7 @@ def launches():
 
 def test_reference_render_vanilla_runs_on_the_cuda_path(ref):
     f = util.golden("frames.npz")
-    coarse, fine = scenes.seed_nets(ref.vanilla.build_nerf, ref_opts.default_opt(use_cuda=True), 1)
+    coarse, fine = scenes.seed_nets(ref.vanilla.build_nerf, nb.default_opt(use_cuda=True), 1)
     assert next(coarse.parameters()).is_cuda and type(coarse).__module__ == "models.vanilla"
     cap = cap_of(ref, f["van_K"], f["van_c2w"], 20, 28)
     l0 = launches()
@@ -68,8 +61,9 @@ def test_reference_render_vanilla_runs_on_the_cuda_path(ref):
     rgb, dep = quiet(ref.render_utils.render_vanilla, coarse, cap, fine_net=None, rays_per_batch=2048, samples_per_ray=64,
                      return_depth=True)
     assert np.abs(rgb - f["cfg1_rgb"]).max() < TOL and np.abs(dep - f["cfg1_depth"]).max() < TOL
-    # a CPU model keeps the reference's own implementation (the golden it produced, up to the host's BLAS rounding)
-    c_cpu, f_cpu = scenes.seed_nets(ref.vanilla.build_nerf, ref_opts.default_opt(use_cuda=False), 1)
+    # a CPU model keeps the reference's own implementation (here its oracle restatement: the golden up to the host's BLAS
+    # rounding)
+    c_cpu, f_cpu = scenes.seed_nets(ref.vanilla.build_nerf, nb.default_opt(use_cuda=False), 1)
     l0 = launches()
     cap = cap_of(ref, f["van_K"], f["van_c2w"], 20, 28)
     rgb = quiet(ref.render_utils.render_vanilla, c_cpu, cap, fine_net=f_cpu, rays_per_batch=100, samples_per_ray=48,
@@ -80,7 +74,7 @@ def test_reference_render_vanilla_runs_on_the_cuda_path(ref):
 def test_reference_human_renderers_run_on_the_cuda_path(ref):
     f = util.golden("frames.npz")
     torch.manual_seed(1)
-    net = quiet(ref.human_nerf.HumanNeRF, ref_opts.default_opt(num_offset_nets=0, use_cuda=True))
+    net = ref.human_nerf.HumanNeRF(nb.default_opt(num_offset_nets=0, use_cuda=False)).cuda()
     scenes.boost_density(net.coarse_human_net)
     sums = [scenes.net_checksum(net.coarse_bkg_net), scenes.net_checksum(net.fine_bkg_net), scenes.net_checksum(net.coarse_human_net)]
     assert np.allclose(sums, f["h_sum"], rtol=1e-6)
@@ -140,221 +134,18 @@ def test_reference_stage_functions_and_forward_on_cuda(ref):
         _, _, iz = ry.ray_to_importance_samples(batch, z, w, 24, device=dev)
         bad = (np.abs(iz.cpu().numpy() - g["i_z"]) > 2e-6).mean()
         assert bad < 0.01                                     # sample_pdf's `denom < 1e-5` discontinuity (see test_gpu_stages.py)
-        coarse, _ = scenes.seed_nets(ref.vanilla.build_nerf, ref_opts.default_opt(use_cuda=True), 1)
+        coarse, _ = scenes.seed_nets(ref.vanilla.build_nerf, nb.default_opt(use_cuda=True), 1)
         l0 = launches()
         out = coarse(torch.from_numpy(g["n_pts"]).to(dev), torch.from_numpy(g["n_views"]).to(dev))
         assert launches() > l0 and np.abs(out.cpu().numpy() - g["n_coarse"]).max() < 1e-3
         # an architecture the kernels do not implement keeps the reference's own forward (install() never changes results)
-        small, _ = scenes.seed_nets(ref.vanilla.build_nerf, ref_opts.default_opt(use_cuda=True, nerf_width=128), 3)
+        small, _ = scenes.seed_nets(ref.vanilla.build_nerf, nb.default_opt(use_cuda=True, nerf_width=128), 3)
         l0 = launches()
         x, v = torch.randn(50, 3, device=dev), torch.nn.functional.normalize(torch.randn(50, 3, device=dev), dim=-1)
         y = small(x, v)
         assert launches() == l0 and y.shape == (50, 4)
-        nofreq, _ = scenes.seed_nets(ref.vanilla.build_nerf, ref_opts.default_opt(use_cuda=True, pos_N_freqs=6, pos_max_freq=5), 3)
+        nofreq, _ = scenes.seed_nets(ref.vanilla.build_nerf, nb.default_opt(use_cuda=True, pos_N_freqs=6, pos_max_freq=5), 3)
         assert nofreq(x, v).shape == (50, 4) and launches() == l0
     # under autograd (training) the reference's torch path runs unless install(train=True)
     out = coarse(torch.from_numpy(g["n_pts"]).to(dev), torch.from_numpy(g["n_views"]).to(dev))
     assert out.requires_grad
-
-
-def _reference_human_trainer_case(ref, device):
-    """The reference's HumanNeRF with per-frame SMPL parameters, assembled as models/human_nerf.py:31-90 does (the SMPL
-    pickle path is hard-coded there to <repo>/data/smplx/smpl, licence-gated and absent: the attributes are set here from a
-    synthetic SMPL-shaped pickle instead), a ray batch through the body, and a stand-in for the trainer object holding the
-    three members HumanNeRFTrainer._eval_human_samples reads (opt, net, val_dataset.scene.captures[i].posed_mesh_cpu)."""
-    import os
-    import tempfile
-    import types
-    from oracle import synth_smpl
-    torch.manual_seed(1)
-    opt = ref_opts.default_opt(num_offset_nets=1, use_cuda=(device == "cuda"), offset_scale=0.02, offset_scale_type="tanh",
-                               samples_per_ray=24, perturb=0.0)
-    net = quiet(ref.human_nerf.HumanNeRF, opt)
-    rng = np.random.RandomState(6)
-    pose, betas = rng.normal(0, 0.3, (1, 72)).astype(np.float32), rng.normal(0, 1, (1, 10)).astype(np.float32)
-    ang = 0.2
-    align = np.eye(4, dtype=np.float32)
-    align[:3, :3] = np.array([[np.cos(ang), 0, np.sin(ang)], [0, 1, 0], [-np.sin(ang), 0, np.cos(ang)]])
-    align = align.T.copy()
-    align[3, :3] = (0.3, -0.1, 2.0)
-    P = torch.nn.Parameter
-    net.poses, net.betas = P(torch.from_numpy(pose).to(device)), P(torch.from_numpy(betas).to(device))
-    net.alignments, net.scale = P(torch.from_numpy(align[None]).to(device)), 0.4
-    pk = os.path.join(tempfile.mkdtemp(), "SMPL_NEUTRAL.pkl")
-    synth_smpl.write_pickle(pk, 0)
-    net.body_model = ref.smpl.SMPL(pk, gender="neutral", device=torch.device(device))
-    da = torch.zeros(24, 3)
-    da[1, 2], da[2, 2] = 1.0, -1.0
-    net.da_smpl = P(da.reshape(1, -1).to(device), requires_grad=False)
-    faces = net.body_model.faces_tensor.cpu()
-    cap = types.SimpleNamespace(posed_mesh_cpu=types.SimpleNamespace(faces_packed=lambda: faces))
-    me = types.SimpleNamespace(opt=opt, net=net, val_dataset=types.SimpleNamespace(scene=types.SimpleNamespace(captures=[cap])))
-    if device == "cpu":
-        # the reference's 'rotate' Embedder puts its frequency matrix on the GPU whenever one is visible, whatever device
-        # the module is meant for (models/vanilla.py:53-56): bring it back for the CPU run of the unpatched reference
-        for j in (net.coarse_human_net, net.coarse_bkg_net, net.fine_bkg_net):
-            for pe in (j.pos_pe, j.dir_pe):
-                if hasattr(pe, "bvals"):
-                    pe.bvals = pe.bvals.cpu()
-    return me, net
-
-
-def test_reference_human_trainer_step_runs_on_the_cuda_path(ref):
-    """install(train=True) under the reference's own HumanNeRFTrainer._eval_human_samples
-    (trainers/human_nerf_trainer.py:241-278) and loss.backward(): ray_to_samples, vertex_forward (SMPL training kernels),
-    warp_samples_to_canonical_diff (device BVH query + blend/inverse kernel), OffsetNet.forward and Joiner.forward (tensor-core
-    training kernels) and their adjoints, against the SAME method of the unpatched reference on the CPU.
-
-    The closest face / point of every sample is a CONSTANT of the step in the reference (libigl's numpy answer, :265-270), and
-    where the closest point lies on an edge both adjacent faces are exact answers: the blended transform is the same for
-    either, but its derivative with respect to the vertices is not (the barycentric formula projects onto the chosen face's
-    plane).  Which one libigl reports is its tie rule (unpinned, DESIGN.md §2), so the CPU run is given the device query's
-    answers: values and gradients are then compared on identical constants."""
-    import importlib
-    import sys
-    tr = importlib.import_module("trainers.human_nerf_trainer")
-    from neuman_b200 import dropin, ops
-    igl_stub = sys.modules["igl"]
-    stub_sd, ops_sd = igl_stub.signed_distance, ops.signed_distance
-    dropin.uninstall()
-    try:
-        me_c, net_c = _reference_human_trainer_case(ref, "cpu")
-        with torch.no_grad():
-            V0 = net_c.vertex_forward(0)[0][0].numpy()
-        rng = np.random.RandomState(3)
-        R = 64
-        eye = V0.mean(0) + np.array([0.0, 0.0, -2.0])
-        d = V0[rng.randint(0, V0.shape[0], R)] + rng.normal(0, 0.01, (R, 3)) - eye
-        dist = np.linalg.norm(d, axis=1, keepdims=True)
-        mk = lambda dev: {"origin": torch.from_numpy(np.repeat(eye[None], R, 0)).float().to(dev),
-                          "direction": torch.from_numpy((d / dist).astype(np.float32)).to(dev),
-                          "human_near": torch.from_numpy(dist - 0.15).float().to(dev),
-                          "human_far": torch.from_numpy(dist + 0.15).float().to(dev), "cur_view_f": torch.tensor(3 / 11), "cap_id": 0}
-        w = torch.from_numpy(rng.normal(0, 1, (R, 24, 3)).astype(np.float32))
-        # ---- the reference's method with the CUDA path installed; the device query's answers are recorded ----
-        nb.install(ref_import.REF_ROOT, train=True)
-        me_g, net_g = _reference_human_trainer_case(ref, "cuda")
-        net_g.load_state_dict(net_c.state_dict())
-        seen = []
-
-        def recording_sd(*a, **k):
-            out = ops_sd(*a, **k)
-            seen.append(tuple(np.asarray(o.cpu() if isinstance(o, torch.Tensor) else o) for o in out))
-            return out
-        ops.signed_distance = recording_sd
-        l0 = launches()
-        out_g = quiet(tr.HumanNeRFTrainer._eval_human_samples, me_g, mk("cuda"), "cuda")
-        ((out_g[3] * w.cuda()).sum() + (out_g[4] * w.flip(0).cuda()).sum()).backward()
-        ops.signed_distance = ops_sd
-        assert launches() - l0 >= 12, "the reference's trainer step did not reach libneuman_b200"
-        assert all(o.is_cuda for o in out_g) and len(seen) == 1
-        # ---- the same method of the unpatched reference on the CPU, on the same closest faces / points ----
-        dropin.uninstall()
-        S_d, I_d, C_d = seen[0]
-        igl_stub.signed_distance = lambda P, V, F, *a, **k: (S_d.astype(np.float64), I_d.astype(np.int32), C_d.astype(np.float64))
-        out_c = quiet(tr.HumanNeRFTrainer._eval_human_samples, me_c, mk("cpu"), "cpu")
-        igl_stub.signed_distance = stub_sd
-        ((out_c[3] * w).sum() + (out_c[4] * w.flip(0)).sum()).backward()
-        assert np.abs(out_g[0].detach().cpu().numpy() - out_c[0].detach().numpy()).max() < 2e-6          # human_pts
-        assert np.abs(out_g[3].detach().cpu().numpy() - out_c[3].detach().numpy()).max() < 1e-5          # can_pts (+ offset)
-        assert np.abs(out_g[4].detach().cpu().numpy() - out_c[4].detach().numpy()).max() < 2e-4          # can_dirs (1 / spacing)
-        assert np.abs(out_g[5].detach().cpu().numpy() - out_c[5].detach().numpy()).max() < 2e-3          # human_out (11-bit operands)
-        for name in ("poses", "betas", "alignments"):
-            g, c = getattr(net_g, name).grad.cpu().numpy(), getattr(net_c, name).grad.numpy()
-            assert np.isfinite(g).all() and np.abs(g - c).max() < 5e-3 * (1 + np.abs(c).max()), (name, np.abs(g - c).max(), np.abs(c).max())
-        g, c = net_g.offset_nets[0].nerf.output_linear.weight.grad.cpu().numpy(), net_c.offset_nets[0].nerf.output_linear.weight.grad.numpy()
-        assert np.abs(g - c).max() < 8e-2 * np.abs(c).max() + 1e-7, (np.abs(g - c).max(), np.abs(c).max())   # tensor-core operands
-        # the device's own query against the reference stub's (float64, exhaustive) on the same points: same distances
-        S_r, I_r, C_r = stub_sd(out_c[0].detach().numpy().astype(np.float64), V0.astype(np.float64), me_c.val_dataset.scene.captures[0].posed_mesh_cpu.faces_packed().numpy())
-        assert np.abs(np.abs(S_d) - np.abs(S_r)).max() < 1e-5
-        # the human network's own gradients come from a loss through its output
-        nb.install(ref_import.REF_ROOT, train=True)
-        net_g.zero_grad()
-        out_g = quiet(tr.HumanNeRFTrainer._eval_human_samples, me_g, mk("cuda"), "cuda")
-        out_g[5].square().mean().backward()
-        assert all(p.grad is not None and torch.isfinite(p.grad).all() for p in net_g.coarse_human_net.parameters())
-        assert net_g.poses.grad is not None and torch.isfinite(net_g.poses.grad).all()
-    finally:
-        ops.signed_distance = ops_sd
-        igl_stub.signed_distance = stub_sd
-        nb.install(ref_import.REF_ROOT)             # back to the module fixture's state (inference drop-in)
-
-
-def _reference_loss_standin(ref, device):
-    """The stand-in trainer of _reference_human_trainer_case extended with what HumanNeRFTrainer.loss_func
-    (trainers/human_nerf_trainer.py:382-446) and its regularisers (:279-380) read: penalties, the canonical-space capture
-    list, the capture's canonical mesh (verts_packed / faces_packed), interval_comp, and the trainer's own methods bound to it."""
-    import importlib
-    import types
-    tr = importlib.import_module("trainers.human_nerf_trainer")
-    me, net = _reference_human_trainer_case(ref, device)
-    for j in (net.coarse_human_net, net.coarse_bkg_net, net.fine_bkg_net):
-        scenes.boost_density(j)                       # default-init densities are <= 0 over the body: the step would re-initialise
-    opt = me.opt
-    opt.white_bkg, opt.importance_samples_per_ray, opt.samples_per_ray = True, 16, 24
-    opt.penalize_outside_factor, opt.dist_exponent = 2.0, 2.0
-    with torch.no_grad():
-        can_v = net.body_model(poses=net.da_smpl, betas=net.betas[0][None], return_tensor=True).detach().cpu()
-    faces = net.body_model.faces_tensor.cpu()
-    me.val_dataset.scene.captures[0].can_mesh = types.SimpleNamespace(verts_packed=lambda: can_v, faces_packed=lambda: faces)
-    K, c2w = scenes.camera(32, 32, seed=5, eye=(0.0, 0.0, -3.0))
-    cam = ref.pinhole_camera.PinholeCamera(32, 32, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
-    me.can_caps = [ref.captures.BasePinholeCapture(cam, ref.camera_pose.CameraPose.from_camera_to_world(c2w.astype(np.float64)))]
-    me.penalize_smpl_alpha, me.penalize_symmetric_alpha, me.penalize_dummy = 0.1, 0.1, 0.0
-    me.penalize_hard_surface, me.penalize_sharp_edge = 0.1, 0.1
-    me.penalize_color_range, me.penalize_outside, me.penalize_mask, me.penalize_lpips = 0.0, 0.0, 0.01, 0.0   # (random dummy directions / LPIPS off)
-    me.interval_comp = 0.8
-    for name in ("_eval_bkg_samples", "_eval_human_samples", "_smpl_symmetry_regularization", "_color_range_regularization",
-                 "_smpl_shape_regularization", "_sparsity_regularization"):
-        setattr(me, name, types.MethodType(getattr(tr.HumanNeRFTrainer, name), me))
-    return tr, me, net
-
-
-def test_reference_human_loss_func_runs_on_the_cuda_path(ref):
-    """The reference's whole HumanNeRFTrainer.loss_func (trainers/human_nerf_trainer.py:382-446: background branch,
-    human branch, symmetry / mask / SMPL-shape / sparsity regularisers, z-sorted merge, RGB loss) with install(train=True),
-    called unmodified, against the same call of the unpatched reference on the CPU; then loss.backward()."""
-    import random
-    from neuman_b200 import dropin
-    dropin.uninstall()
-    try:
-        tr, me_c, net_c = _reference_loss_standin(ref, "cpu")
-        with torch.no_grad():
-            V0 = net_c.vertex_forward(0)[0][0].numpy()
-        rng = np.random.RandomState(3)
-        R = 64
-        eye = V0.mean(0) + np.array([0.0, 0.0, -2.0])
-        d = V0[rng.randint(0, V0.shape[0], R)] + rng.normal(0, 0.01, (R, 3)) - eye
-        dist = np.linalg.norm(d, axis=1, keepdims=True)
-        is_hit = (rng.uniform(size=R) < 0.8).astype(np.int64)
-        color = rng.uniform(size=(R, 3))
-        f = lambda a: torch.from_numpy(np.asarray(a)).float()[None]
-
-        def mk():                                    # a DataLoader batch (leading axis 1, CPU tensors), datasets/human_rays.py:233-247
-            return {"origin": f(np.repeat(eye[None], R, 0)), "direction": f(d / dist), "human_near": f(dist - 0.15),
-                    "human_far": f(dist + 0.15), "bkg_near": f(np.full((R, 1), 0.5)), "bkg_far": f(np.full((R, 1), 4.0)),
-                    "color": f(color), "is_bkg": torch.from_numpy(1 - is_hit)[None], "is_hit": torch.from_numpy(is_hit)[None],
-                    "cur_view_f": torch.tensor([3 / 11]), "cur_view": torch.tensor([3]), "cap_id": torch.tensor([0]),
-                    "patch_counter": torch.tensor([0])}
-        random.seed(0)
-        np.random.seed(0)
-        ld_c = quiet(tr.HumanNeRFTrainer.loss_func, me_c, mk())
-        nb.install(ref_import.REF_ROOT, train=True)
-        _, me_g, net_g = _reference_loss_standin(ref, "cuda")
-        net_g.load_state_dict(net_c.state_dict())
-        random.seed(0)
-        np.random.seed(0)
-        l0 = launches()
-        ld_g = quiet(tr.HumanNeRFTrainer.loss_func, me_g, mk())
-        assert launches() - l0 >= 30, "the reference's loss_func did not reach libneuman_b200"
-        assert float(ld_c["fine_rgb_loss"]) > 1e-3 and float(ld_c["smpl_shape_reg"]) > 1e-3       # a live step, not the re-init branch
-        for k, v in ld_c.items():
-            g, c = float(ld_g[k]), float(v)
-            assert abs(g - c) < 2e-2 * abs(c) + 2e-5, (k, g, c)
-        total = sum(ld_g.values())
-        total.backward()
-        for p in list(net_g.coarse_human_net.parameters()) + list(net_g.offset_nets.parameters()) + [net_g.poses, net_g.betas, net_g.alignments]:
-            assert p.grad is not None and torch.isfinite(p.grad).all()
-        assert float(net_g.poses.grad.abs().max()) > 0 and float(net_g.coarse_human_net.nerf.alpha_linear.weight.grad.abs().max()) > 0
-    finally:
-        nb.install(ref_import.REF_ROOT)

@@ -8,7 +8,7 @@ mean on a given configuration, both stored next to the golden (per ray, same ray
             renderers sort background and human samples by depth, so an ulp moves a sample across another one and changes
             the pixel by O(1e-4..1e-3); the fp32 reference is only defined up to that.
   floor16 = |fp32 algorithm - fp32 algorithm with the nets' matmul operands rounded to 11 significand bits|: what any
-            tensor-core evaluation (tcgen05 kind::f16 or kind::tf32) does to the result, independent of the kernel.
+            tensor-core evaluation (fp16 or tf32 operands) does to the result, independent of the kernel.
 The fp32 CUDA-core mode (NM_MLP_SIMT_F32) is held to max(1e-4, K64 * floor64); the tensor-core mode (the default and the
 benchmarked one) to max(1e-4, K16 * max(floor16, floor64)), with K = 2 on the 99.5th percentile and K = 8 on the maximum
 (the floors are ONE realisation of the rounding noise, not a bound: the tails are sample flips across a discontinuity --

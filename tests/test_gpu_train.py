@@ -55,7 +55,7 @@ def _rel(a, b):
 
 @pytest.mark.parametrize("n", [1, 63, 64, 1000, 4173, 64 * 74 * 3 + 5])
 def test_dw_gemm(n):
-    """k_dw_gemm (TMA-fed MN-major tcgen05 GEMMs, K = n) against fp32 matmuls of the same fp16 planes: fp32
+    """k_dw_gemm (TMA-fed MN-major wgmma GEMMs, K = n) against fp32 matmuls of the same fp16 planes: fp32
     accumulation in a different order -> 1e-4 relative L2; rows 128.. of the views item stay zero."""
     from neuman_b200 import ops
     from neuman_b200.ops import _p

@@ -1,6 +1,6 @@
 """The human trainer's forward / adjoint kernels (neuman_b200/csrc/human_train_kernels.cuh, smpl_train_kernels.cuh)
 executed on the host by the serial emulation in tests/emu/ -- the SAME kernel bodies libneuman_b200.so compiles for
-sm_100a -- against torch autograd of the oracle restatement of the reference's lines (utils/ray_utils.py:69-93,
+sm_90a -- against torch autograd of the oracle restatement of the reference's lines (utils/ray_utils.py:69-93,
 trainers/human_nerf_trainer.py:263-276, models/human_nerf.py:92-122, models/smpl.py:266-505).  This is the CPU half of
 the parity check (no GPU in the build container); tests/test_gpu_human_train.py repeats it through the CUDA library."""
 import ctypes as C

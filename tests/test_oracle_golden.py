@@ -1,12 +1,23 @@
 """Pins the oracle (oracle/neuman_oracle.py) to the committed golden vectors, which were produced by
 the unmodified reference (tools/make_golden.py).  Runs anywhere (no GPU, no reference tree)."""
 import numpy as np
+import pytest
 import torch
 
 from oracle import neuman_oracle as no
 from tests import util
 
 TOL = 2e-6
+
+
+@pytest.fixture(autouse=True, scope="module")
+def _one_thread():
+    """CPU float32 reductions round differently with the number of threads they are split over: compare on one thread,
+    so that the results do not depend on the host's core count"""
+    n = torch.get_num_threads()
+    torch.set_num_threads(1)
+    yield
+    torch.set_num_threads(n)
 
 
 def test_networks_have_reference_weights():

@@ -1,6 +1,6 @@
 """CPU emulation of the warp stage's packet BVH traversal (neuman_b200/csrc/warp.cu: LBVH build, bvh_nearest_face): counts
 internal-node visits, triangle tests and stack pops per 32-lane packet for the packet shapes of k_warp_nearest, on the
-hit rays of the cfg4/cfg5 body.  Used for profiles/r02_configs.md (why the stage is instruction-bound).
+hit rays of the cfg4/cfg5 body.
 python tools/bvh_visits.py"""
 import sys, os
 import numpy as np

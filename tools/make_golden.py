@@ -1,4 +1,4 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (imported from /root/reference,
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (imported from $NEUMAN_REFERENCE,
 oracle/ref_import.py) on seeded synthetic inputs.  Run in the build container only:
 
     python tools/make_golden.py

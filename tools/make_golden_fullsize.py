@@ -1,5 +1,5 @@
 """Generates tests/golden/fullsize.npz: BASELINE.json configurations 2-5 at their stated sizes, rendered by the
-UNMODIFIED reference (imported from /root/reference through oracle/ref_import.py) on one 64x64 pixel block (4096 rays)
+UNMODIFIED reference (imported from $NEUMAN_REFERENCE through oracle/ref_import.py) on one 64x64 pixel block (4096 rays)
 per configuration that straddles a body silhouette.  Run in the build container only:
 
     python tools/make_golden_fullsize.py [cfg2 cfg3 cfg4 cfg5]
@@ -9,7 +9,7 @@ is shifted by the block origin (neuman_b200.synthetic.window_camera): exactly th
 Next to every reference output the file stores the measured noise floors on the same rays (SURVEY.md §8d):
   floor64_* : max |fp32 oracle - the same algorithm carried in float64|   (the reference's own rounding noise)
   floor16_* : max |fp32 oracle - fp32 oracle with the MLP's matmul operands rounded to 11 significand bits|
-              (what ANY tensor-core evaluation of the nets -- tcgen05 kind::f16 or kind::tf32 -- does to the result)
+              (what ANY tensor-core evaluation of the nets -- fp16 or tf32 operands -- does to the result)
 and `grazing`, the rays whose hit/miss decision or colour is ill-conditioned (|far - near| < 1e-3 for an actor).
 """
 import contextlib

@@ -17,7 +17,7 @@ from oracle import scenes                     # noqa: E402
 mode_name = sys.argv[1] if len(sys.argv) > 1 else "tc"
 n_big = int(sys.argv[2]) if len(sys.argv) > 2 else 4 * 1024 * 1024
 mode = {"simt": _lib.NM_MLP_SIMT_F32, "tc": _lib.NM_MLP_TC_F16}[mode_name]
-print("mode", mode_name, "pair", os.environ.get("NEUMAN_TC_PAIR", "2"), flush=True)
+print("mode", mode_name, flush=True)
 coarse, fine = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False), 1)
 human, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False, posenc="rotate"), 2)
 for name, net in (("posenc", coarse), ("rotate", human)):
