@@ -73,7 +73,7 @@ typedef struct {
   float dir_min_freq, dir_max_freq; int32_t dir_n_freqs;   /* options/options.py:67-69 */
 } nm_nerf_desc;
 
-/* Re-pack the weights of one Joiner into the kernel layouts (fp16 UMMA tiles + fp32 transposed).
+/* Re-pack the weights of one Joiner into the kernel layouts (fp16 wgmma slabs + fp32 transposed).
  * Replaces nothing in the reference; it is the cost of `net.cuda()` / checkpoint load. */
 int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* desc, void* stream);
 
@@ -129,10 +129,6 @@ int nm_pe_backward(nm_ctx* ctx, int slot, int32_t which, const float* x, int64_t
  * loss scale of the g planes. */
 int nm_dw_gemm(nm_ctx* ctx, const void* g_pre, const void* g_f, const void* g_v, const void* stash_x,
                const void* stash_f, int64_t n, float* out, float* bias_out, void* stream);
-
-/* Bias gradients (the `.bias.grad` torch autograd accumulates): out[p][c] = sum_i src[p][i][c] over fp16 planes
- * src [planes][n][width] (width even, <= 256), fp32 accumulation.  out is overwritten. */
-int nm_colsum_f16(nm_ctx* ctx, const void* src, int32_t planes, int64_t n, int32_t width, float* out, void* stream);
 
 /* Same network, but the sample positions are generated in-kernel: pts[r,s] = o[r] + d[r]*z[r,s],
  * views = d[r] (utils/ray_utils.py:131-132).  o,d: [R,3]; z: [R,S]; raw: [R,S,4]. */

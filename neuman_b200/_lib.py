@@ -60,7 +60,6 @@ SIGNATURES = {
     "nm_mlp_backward": (C.c_int, [_P, C.c_int, _P, _P, _I64, _P, _P, _P, _P, _P, _P]),
     "nm_pe_backward": (C.c_int, [_P, C.c_int, _I32, _P, _I64, _P, _I32, _P, _I64, _P, _P]),
     "nm_dw_gemm": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _P, _P, _P]),
-    "nm_colsum_f16": (C.c_int, [_P, _P, _I32, _I64, _I32, _P, _P]),
     "nm_mlp_forward_rays": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _I64, _I32, _P, _P]),
     "nm_raygen": (C.c_int, [_P, C.POINTER(NmCamera), C.c_int, _I64, _I64, _P, _P, _P, _P]),
     "nm_near_far": (C.c_int, [_P, _P, _P, _I64, _P, _I32, _F, _P, _P, _P]),

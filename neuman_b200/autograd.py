@@ -2,7 +2,6 @@
 trainers/vanilla_nerf_trainer.py:45-96, trainers/human_nerf_trainer.py:382-446).  Forward = the same CUDA
 kernels as inference; backward = their CUDA adjoints.  CUDA tensors only."""
 import ctypes as C
-import os
 
 import torch
 
@@ -60,10 +59,6 @@ def _mm32(a, b):
     return torch.mm(a, b, out_dtype=torch.float32)
 
 
-def _use_torch_chain():
-    return os.environ.get("NEUMAN_BWD_TORCH", "0") == "1"
-
-
 class _JoinerMLP(torch.autograd.Function):
     """forward: k_mlp_tc<.., kTrain> (csrc/mlp_tc.cu) = the inference kernel + an fp16 stash of every layer
     output and the ReLU sign words.
@@ -75,7 +70,8 @@ class _JoinerMLP(torch.autograd.Function):
     Gradients go to the network parameters and, when they require grad, to the sample positions / directions
     (dL/d encoding by two small cuBLAS GEMMs on the gradient planes, then k_pe_backward), which is what the human
     trainer's differentiable warp and offset nets consume (trainers/human_nerf_trainer.py:241-278).
-    NEUMAN_BWD_TORCH=1 evaluates the same chain with torch GEMMs from the same stash (debug / cross-check).
+    The two kernel launches sit behind module-level functions (_chain_kernel, _dw_kernel), so that a test can put a
+    torch restatement of the same chain in their place (tests/util.py).
 
     The gradient is the exact adjoint of the fp16-operand forward: ReLU masks are those of the fp16 activations,
     so it differs from an fp32 forward's gradient where a pre-activation changes sign under the rounding
@@ -127,8 +123,7 @@ class _JoinerMLP(torch.autograd.Function):
             grads = {k: torch.zeros_like(v) for k, v in P.items()}
             d_pts, d_views = torch.zeros_like(pts), torch.zeros_like(views)
         else:
-            chain = _chain_torch if _use_torch_chain() else _chain_kernel
-            g_pre, g_f, g_v, inv = chain(joiner, P, stash, g)
+            g_pre, g_f, g_v, inv = _chain_kernel(joiner, P, stash, g)
             grads = _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv) if need_w else {}
             if fctx.needs_input_grad[0]:
                 d_pts = _input_grad(joiner, P, pts, 0, ((g_pre[0], 'pts_linears.0.weight', 0), (g_pre[5], 'pts_linears.5.weight', 0)), inv)
@@ -156,14 +151,6 @@ def _input_grad(joiner, P, x, which, terms, inv):
     d_x = torch.empty(n, 3, device=x.device, dtype=torch.float32)
     ctx.check(ctx.lib.nm_pe_backward(ctx.h, slot, which, _p(x), 0, _p(d_enc), ld, _p(inv.contiguous()), n, _p(d_x), ctx.stream()))
     return d_x
-
-
-def _colsum(ctx, t):
-    """[planes, n, width] fp16 -> [planes, width] fp32 column sums (csrc/mlp_tc_bwd.cu: k_colsum_f16)."""
-    planes, n, width = t.shape
-    out = torch.empty(planes, width, device=t.device, dtype=torch.float32)
-    ctx.check(ctx.lib.nm_colsum_f16(ctx.h, _p(t), planes, n, width, _p(out), ctx.stream()))
-    return out
 
 
 def _encodings(joiner, pts, views):
@@ -199,20 +186,7 @@ def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
     gvt = g_v.t()
     wd = _mm32(gvt, sdpe) * inv                                           # [128, 32]
     w0 = _mm32(g_pre[0].t(), spe) * inv                                   # [256,64]: column 63 = bias gradient (1.0 channel)
-    if os.environ.get("NEUMAN_DW_TORCH", "0") == "1":                     # cross-check path: cuBLAS GEMMs + column-sum kernel
-        dw = torch.zeros(9, 256, 256, device=g.device, dtype=torch.float32)
-        for k in range(7):
-            dw[k] = _mm32(g_pre[k + 1].t(), sx[k])
-        dw[7] = _mm32(g_f.t(), sx[7])
-        dw[8, :128] = _mm32(gvt, sf)
-        db = torch.zeros(9, 256, device=g.device, dtype=torch.float32)
-        db[:7] = _colsum(ctx, g_pre)[1:]
-        db[7] = _colsum(ctx, g_f[None])[0]
-        db[8, :128] = _colsum(ctx, g_v[None])[0]
-    else:                                                                 # k_dw_gemm: every plane read once at HBM rate
-        dw = torch.empty(9, 256, 256, device=g.device, dtype=torch.float32)
-        db = torch.empty(9, 256, device=g.device, dtype=torch.float32)
-        ctx.check(ctx.lib.nm_dw_gemm(ctx.h, _p(g_pre), _p(g_f), _p(g_v), _p(sx), _p(sf), g.shape[0], _p(dw), _p(db), ctx.stream()))
+    dw, db = _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, g.shape[0])
     dw, db = dw * inv, db * inv
     grads['views_linears.0.weight'] = torch.cat([dw[8, :128], wd[:, :n_dpe]], 1)
     grads['views_linears.0.bias'] = db[8, :128]
@@ -242,27 +216,14 @@ def _chain_kernel(joiner, P, stash, g):
     return g_pre, g_f, g_v, 1.0 / scale
 
 
-def _chain_torch(joiner, P, stash, g):
-    """The chain of k_mlp_tc_bwd restated with torch GEMMs on the same stash (same masks, same fp16 rounding
-    points): the cross-check of the kernel in tests/test_gpu_train.py."""
-    sx, sf, sv, sm = stash
-    n_pe = joiner.pos_pe.out_dim
-    scale = _pow2_scale(g, 256.0)
-    inv = 1.0 / scale
-
-    def wh(name):
-        return P[name].detach().half()
-    gs = g * scale
-    g_v = ((gs[:, :3] @ P['rgb_linear.weight'].detach().float()) * (sv > 0)).half()
-    g_f = _mm32(g_v, wh('views_linears.0.weight')[:, :256].contiguous()).half()
-    dX = _mm32(g_f, wh('feature_linear.weight')) + gs[:, 3:4] * P['alpha_linear.weight'].detach().float()
-    g_pre = torch.empty_like(sx)
-    for l in range(7, -1, -1):
-        g_pre[l] = (dX * (sx[l] > 0)).half()
-        if l > 0:
-            w = wh('pts_linears.%d.weight' % l)
-            dX = _mm32(g_pre[l], w[:, n_pe:].contiguous() if l == 5 else w)
-    return g_pre, g_f, g_v, inv
+def _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, n):
+    """The nine 256-wide weight gradients and their bias gradients, still carrying the loss scale of the g planes: one
+    k_dw_gemm launch (csrc/dw_gemm.cu), every gradient and stash plane read once.
+    -> dw [9,256,256], db [9,256] fp32 (plane 8: rows 0..127 used)."""
+    dw = torch.empty(9, 256, 256, device=g_pre.device, dtype=torch.float32)
+    db = torch.empty(9, 256, device=g_pre.device, dtype=torch.float32)
+    ctx.check(ctx.lib.nm_dw_gemm(ctx.h, _p(g_pre), _p(g_f), _p(g_v), _p(sx), _p(sf), n, _p(dw), _p(db), ctx.stream()))
+    return dw, db
 
 
 def joiner_forward(joiner, input_pts, input_views):

@@ -39,9 +39,7 @@ static void free_mesh(NmMesh& m) {
   if (m.verts) cudaFree(m.verts);
   if (m.faces) cudaFree(m.faces);
   if (m.T) cudaFree(m.T);
-  if (m.tri_sphere) cudaFree(m.tri_sphere);
-  if (m.cell_start) cudaFree(m.cell_start);
-  if (m.cell_tris) cudaFree(m.cell_tris);
+  if (m.bvh) cudaFree(m.bvh);
   if (m.vnorm) cudaFree(m.vnorm);
   if (m.adj) cudaFree(m.adj);
   if (m.pn_tmp) cudaFree(m.pn_tmp);
@@ -115,19 +113,9 @@ extern "C" int nm_last_render_stats(const nm_ctx* ctx, int64_t* mlp_evals, int64
 }
 
 int nm_impl_workspace(nm_ctx* ctx, size_t bytes, char** out) {
-  if (bytes > ctx->ws_bytes) {
-    if (ctx->ws) {
-      NM_CHECK_CUDA(ctx, cudaDeviceSynchronize());
-      NM_CHECK_CUDA(ctx, cudaFree(ctx->ws));
-      ctx->ws = nullptr;
-      ctx->ws_bytes = 0;
-    }
-    size_t want = bytes + (bytes >> 3);
-    NM_CHECK_CUDA(ctx, cudaMalloc(&ctx->ws, want));
-    ctx->ws_bytes = want;
-  }
+  const int rc = ensure(ctx, &ctx->ws, &ctx->ws_bytes, bytes);
   *out = ctx->ws;
-  return NM_OK;
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -384,14 +372,6 @@ extern "C" int nm_dw_gemm(nm_ctx* ctx, const void* g_pre, const void* g_f, const
   if (!g_pre || !g_f || !g_v || !stash_x || !stash_f) NM_FAIL(ctx, NM_ERR_INVALID, "nm_dw_gemm: null argument");
   return nm_impl_dw_gemm(ctx, (const __half*)g_pre, (const __half*)g_f, (const __half*)g_v, (const __half*)stash_x,
                          (const __half*)stash_f, n, out, bias_out, (cudaStream_t)stream);
-}
-
-extern "C" int nm_colsum_f16(nm_ctx* ctx, const void* src, int32_t planes, int64_t n, int32_t width, float* out, void* stream) {
-  NM_ENTER(ctx);
-  if (planes < 0 || n < 0 || width <= 0 || width > 256 || (width & 1)) NM_FAIL(ctx, NM_ERR_INVALID, "nm_colsum_f16: bad shape");
-  if (planes == 0) return NM_OK;
-  if (!out || (n > 0 && !src)) NM_FAIL(ctx, NM_ERR_INVALID, "nm_colsum_f16: null argument");
-  return nm_impl_colsum_f16(ctx, (const __half*)src, planes, n, width, out, (cudaStream_t)stream);
 }
 
 extern "C" int nm_mlp_forward_rays(nm_ctx* ctx, int slot, int mode, const float* origins, const float* dirs,

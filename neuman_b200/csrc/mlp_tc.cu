@@ -77,7 +77,7 @@ struct TcParams {
   const float* consts;      // device constant table (TC_CONST_FLOATS)
   long long n_tiles;        // number of 128-sample tiles
   int32_t* range_flag;      // device word: bit 0 is set when an activation reached the fp16 range limit (saturated)
-  int range_phase;          // sampled range check (kRange == 1): the rounds r with r % 64 == range_phase % 64 are checked
+  int range_phase;          // sampled range check: the rounds r with r % 64 == range_phase % 64 are checked
   // training forward (kTrain): fp16 activation stash for the backward pass, planes of n rows each
   __half* st_x;             // [8][n][256] post-ReLU outputs of layers 0..7
   __half* st_f;             // [n][256]    feature_linear output
@@ -221,7 +221,7 @@ __device__ __forceinline__ void quad_or(uint32_t (&w)[8]) {
 // ---------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------
-template <bool kTrain, int kRange>
+template <bool kTrain>
 __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
   using C = TcCfg;
   constexpr int SLABS = tc_slabs_per_tile();
@@ -272,7 +272,7 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
   for (long long it = 0; it < my_tiles; ++it) {
     const long long tile = blockIdx.x + it * gridDim.x;
     const long long row0 = tile * 128 + wg * TC_WG_ROWS;          // first sample of this warpgroup
-    const bool track = kRange == 2 || (kRange == 1 && (it % rperiod) == (P.range_phase % rperiod));
+    const bool track = (it % rperiod) == (P.range_phase % rperiod);
     // ---- encodings (Embedder.forward, models/vanilla.py:82-92): threads 0-63 position, 64-127 direction of row wtid % 64 ----
     {
       const int r = wtid & 63;
@@ -286,7 +286,7 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
         encode_f16(P.dir_pe, v, e, 12);
         store_row_swizzled(wbuf + C::OFF_DIR, r, e, 4);
       }
-      if (kRange && track) { track_range<false>(rng, e[0]); track_range<false>(rng, e[1]); }   // raw x, y, z (+ one sine)
+      if (track) { track_range<false>(rng, e[0]); track_range<false>(rng, e[1]); }   // raw x, y, z (+ one sine)
       fence_async_smem();
       wg_sync(wg);
     }
@@ -371,7 +371,7 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
       }
     }
   }
-  if (kRange && (((rng & 0xFFFFu) >= 0x7BFFu) || ((rng >> 16) >= 0x7BFFu))) atomicOr(P.range_flag, 1);
+  if (((rng & 0xFFFFu) >= 0x7BFFu) || ((rng >> 16) >= 0x7BFFu)) atomicOr(P.range_flag, 1);
   if (kTrain && wtid == 0) tma_store_wait_all();
 }
 
@@ -478,8 +478,6 @@ static TcPlan make_plan() {
   return p;
 }
 
-bool nm_tc_available() { return true; }
-
 int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   TcPlan plan = make_plan();
   const size_t halfs = plan.image_bytes / 2;
@@ -502,12 +500,12 @@ int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   return NM_OK;
 }
 
-template <bool kTrain, int kRange>
+template <bool kTrain>
 static int launch_tc(nm_ctx* ctx, const TcParams& P, cudaStream_t st) {
-  NM_SET_SMEM_ONCE(ctx, (k_mlp_tc<kTrain, kRange>), TcCfg::SMEM_BYTES);
+  NM_SET_SMEM_ONCE(ctx, k_mlp_tc<kTrain>, TcCfg::SMEM_BYTES);
   long long ctas = ctx->sm_count;
   if (P.n_tiles < ctas) ctas = P.n_tiles > 0 ? P.n_tiles : 1;
-  k_mlp_tc<kTrain, kRange><<<(unsigned)ctas, TcCfg::THREADS, TcCfg::SMEM_BYTES, st>>>(P);
+  k_mlp_tc<kTrain><<<(unsigned)ctas, TcCfg::THREADS, TcCfg::SMEM_BYTES, st>>>(P);
   NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }
@@ -536,15 +534,5 @@ int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
         tc_make_store_map(&P.map_v, stash->v, 1, (uint64_t)n, 128))
       NM_FAIL(ctx, NM_ERR_CUDA, "nm_mlp_forward_train: cuTensorMapEncodeTiled failed");
   }
-  // NEUMAN_TC_RANGE: 0 = no range flag, 1 (default) = sampled (every 64th round, rotating phase), 2 = every sample
-  static const int range_mode = [] { const char* e = getenv("NEUMAN_TC_RANGE"); return e ? atoi(e) : 1; }();
-#define NM_LAUNCH(TRAIN)                                                  \
-  do {                                                                    \
-    if (range_mode <= 0) return launch_tc<TRAIN, 0>(ctx, P, st);          \
-    if (range_mode == 1) return launch_tc<TRAIN, 1>(ctx, P, st);          \
-    return launch_tc<TRAIN, 2>(ctx, P, st);                               \
-  } while (0)
-  if (P.st_x) NM_LAUNCH(true);
-  NM_LAUNCH(false);
-#undef NM_LAUNCH
+  return stash ? launch_tc<true>(ctx, P, st) : launch_tc<false>(ctx, P, st);
 }

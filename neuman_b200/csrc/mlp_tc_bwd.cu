@@ -235,44 +235,6 @@ __global__ void k_bw_pack(BwPackSrc S, uint32_t image_bytes, __half* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------
-// Bias gradients: column sums of fp16 gradient planes, fp32 accumulation.  HBM-bound (reads each plane once).
-// grid = (row chunks, planes); a block owns `width` columns (2 per thread) and strides over its rows.
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_colsum_f16(const __half* __restrict__ src, long long n, int width,
-                                                    long long rows_per_block, float* __restrict__ out) {
-  const int plane = blockIdx.y;
-  const long long r0 = (long long)blockIdx.x * rows_per_block;
-  const long long r1 = min(n, r0 + rows_per_block);
-  const int c2 = threadIdx.x;                       // column pair
-  if (2 * c2 >= width) return;
-  const __half2* p = reinterpret_cast<const __half2*>(src + ((size_t)plane * n + r0) * width) + c2;
-  const size_t stride = (size_t)width / 2;
-  float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
-  long long r = r0;
-  for (; r + 4 <= r1; r += 4) {                     // 4 independent loads in flight per thread
-    const float2 v0 = __half22float2(p[0]), v1 = __half22float2(p[stride]);
-    const float2 v2 = __half22float2(p[2 * stride]), v3 = __half22float2(p[3 * stride]);
-    a0 += v0.x; a1 += v0.y; b0 += v1.x; b1 += v1.y;
-    a0 += v2.x; a1 += v2.y; b0 += v3.x; b1 += v3.y;
-    p += 4 * stride;
-  }
-  for (; r < r1; ++r) { const float2 v = __half22float2(p[0]); a0 += v.x; a1 += v.y; p += stride; }
-  atomicAdd(out + (size_t)plane * width + 2 * c2, a0 + b0);
-  atomicAdd(out + (size_t)plane * width + 2 * c2 + 1, a1 + b1);
-}
-
-int nm_impl_colsum_f16(nm_ctx* ctx, const __half* src, int planes, int64_t n, int width, float* out, cudaStream_t st) {
-  NM_CHECK_CUDA(ctx, cudaMemsetAsync(out, 0, (size_t)planes * width * sizeof(float), st));
-  const int chunks = max(1, (ctx->sm_count * 16) / max(planes, 1));
-  long long rows_per_block = (n + chunks - 1) / chunks;
-  if (rows_per_block < 64) rows_per_block = 64;
-  dim3 grid((unsigned)((n + rows_per_block - 1) / rows_per_block), planes);
-  k_colsum_f16<<<grid, 128, 0, st>>>(src, n, width, rows_per_block, out);
-  NM_CHECK_LAUNCH(ctx);
-  return NM_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
 // Adjoint of Embedder.forward (models/vanilla.py:82-92): d_x = J^T d_enc with
 //   posenc: enc = [x, sin(f_k x), cos(f_k x)]_k          rotate: enc = [x, sin(x B^T), cos(x B^T)]
 // One thread per sample; sin/cos recomputed in fp32 exactly as the fp32 forward does (nm_pe_pair).

@@ -17,8 +17,8 @@
 #define NM_RANGE_FLAG_WORD 32  // word of ctx->d_counter the tensor-core kernels OR their range flag into
 
 // ---- packed network ------------------------------------------------------------------------
-// fp32 transposed weights ([in_padded][out]) for the SIMT kernel and fp16 UMMA-tiled weights for
-// the tensor-core kernel live in one device allocation per slot.
+// fp32 transposed weights ([in_padded][out]) for the SIMT kernel live in one device allocation per slot; the
+// tensor-core kernels read fp16 slabs in the 128B-swizzled wgmma layout from their own allocations.
 struct NmNet {
   bool packed = false;
   nm_nerf_desc desc{};
@@ -45,15 +45,10 @@ struct NmMesh {
   float* verts = nullptr;      // [V,3] f32
   int32_t* faces = nullptr;    // [F,3]
   double* T = nullptr;         // [n_T,16] f64
-  // acceleration grid (warp.cu)
-  float4* tri_sphere = nullptr;   // [F] centroid xyz + radius
-  int32_t* cell_start = nullptr;  // [ncell+1]
-  int32_t* cell_tris = nullptr;   // [n_refs]
-  int32_t n_refs = 0;
-  float3 grid_min = {0, 0, 0};
-  float cell = 0.f;
-  int3 dims = {0, 0, 0};
-  size_t cap_refs = 0, cap_cells = 0, cap_verts = 0, cap_faces = 0, cap_T = 0;
+  size_t cap_verts = 0, cap_faces = 0, cap_T = 0;
+  // closest-face queries (warp.cu): one device block holds the LBVH and its build buffers (warp.cu: bvh_layout)
+  char* bvh = nullptr;
+  size_t cap_bvh = 0;             // bytes
   // near/far culling (rays.cu): vertices in Morton order, 32 per group, one bounding sphere per group
   float4* vsorted = nullptr;      // [n_vgroups * 32] (x, y, z, 0); the tail of the last group repeats its first vertex
   float4* vgroup = nullptr;       // [n_vgroups] centre + radius
@@ -147,6 +142,19 @@ struct NmDeviceGuard {
     NM_CHECK_CUDA(ctx, cudaGetLastError());  \
   } while (0)
 
+// Grow-only device buffer: *p holds at least `need` elements of T afterwards (*cap = its capacity).  Growing
+// synchronises the device before the free, since work already queued on any stream may still read the old buffer,
+// and reserves 1/8 more than asked so that slowly growing sizes do not reallocate every call.
+template <typename T>
+static int ensure(nm_ctx* ctx, T** p, size_t* cap, size_t need) {
+  if (need <= *cap && *p) return NM_OK;
+  if (*p) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(*p)); *p = nullptr; }
+  const size_t want = need + (need >> 3) + 16;
+  NM_CHECK_CUDA(ctx, cudaMalloc(p, want * sizeof(T)));
+  *cap = want;
+  return NM_OK;
+}
+
 // torch.linspace(0, 1, steps) element i in float32: ATen computes start + i*step for the first half
 // and end - (steps-1-i)*step for the second half, step = (end-start)/(steps-1).
 // Compile units that use this are built with -fmad=false so nothing is contracted.
@@ -182,17 +190,15 @@ struct NmTrainStash {
   __half* x;     // [8][n][256] post-ReLU outputs of pts_linears 0..7
   __half* f;     // [n][256]    feature_linear output
   __half* v;     // [n][128]    views layer post-ReLU
-  uint32_t* m;   // [9][n][8]   ReLU sign words: planes 0..7 pts_linears, plane 8 views layer (16 bits per 16 columns, mlp_tc.cu epi_sub16)
+  uint32_t* m;   // [9][n][8]   ReLU sign words: planes 0..7 pts_linears, plane 8 views layer (16 bits per 16 columns, mlp_tc.cu fwd_epi)
 };
 int nm_impl_pe_backward(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64_t group, const float* d_enc, int ld,
                         const float* inv_scale, int64_t n, float* d_x, cudaStream_t st);
 int nm_tc_encode(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64_t group, int64_t n, __half* out, cudaStream_t st);
 int nm_impl_dw_gemm(nm_ctx* ctx, const __half* g_pre, const __half* g_f, const __half* g_v, const __half* st_x,
                     const __half* st_f, int64_t n, float* out, float* bias_out, cudaStream_t st);
-int nm_impl_colsum_f16(nm_ctx* ctx, const __half* src, int planes, int64_t n, int width, float* out, cudaStream_t st);
 int nm_tc_backward(nm_ctx* ctx, NmNet& net, const float* d_raw, const float* scale, int64_t n, const __half* st_v,
                    const uint32_t* st_m, __half* g_pre, __half* g_f, __half* g_v, cudaStream_t st);
 int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
                   const float* origins, const float* dirs, const float* z, int64_t n,
                   int32_t group, float* raw, cudaStream_t st, const NmTrainStash* stash = nullptr);
-bool nm_tc_available();

@@ -13,8 +13,6 @@
 #include "nm_internal.cuh"
 #include "smpl_train_kernels.cuh"
 
-#define SMPL_MAX_J 64
-
 // v_shaped = v_template + shapedirs . beta     (blend_shapes, models/smpl.py:383)
 __global__ void k_smpl_shape(const float* __restrict__ v_template, const float* __restrict__ shapedirs,
                              const float* __restrict__ betas, int nv, int nb, float* __restrict__ v_shaped) {
@@ -41,39 +39,20 @@ __global__ void __launch_bounds__(256) k_smpl_joints(const float* __restrict__ J
   if (threadIdx.x == 0) J[3 * j + c] = red[0];
 }
 
-struct SmplParents { int p[SMPL_MAX_J]; };
-
 // Rodrigues + kinematic chain + relative transforms A_j (models/smpl.py:407-438, :454-505). One thread.
-__global__ void k_smpl_chain(const float* __restrict__ pose, const float* __restrict__ J, SmplParents par, int nj,
+__global__ void k_smpl_chain(const float* __restrict__ pose, const float* __restrict__ J, SmpltParents par, int nj,
                              float* __restrict__ A) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  float G[SMPL_MAX_J][16];
+  float G[SMPLT_MAX_J][16];
   for (int j = 0; j < nj; ++j) {
-    float rx = pose[3 * j], ry = pose[3 * j + 1], rz = pose[3 * j + 2];
-    float ax = rx + 1e-8f, ay = ry + 1e-8f, az = rz + 1e-8f;                       // (:422)
-    float angle = sqrtf(ax * ax + ay * ay + az * az);
-    float dx = rx / angle, dy = ry / angle, dz = rz / angle;
-    float s = sinf(angle), c = cosf(angle);
-    float K[9] = {0.f, -dz, dy, dz, 0.f, -dx, -dy, dx, 0.f};
-    float K2[9];
-    for (int a = 0; a < 3; ++a)
-      for (int b = 0; b < 3; ++b) K2[3 * a + b] = K[3 * a] * K[b] + K[3 * a + 1] * K[3 + b] + K[3 * a + 2] * K[6 + b];
     float L[16];
-    for (int a = 0; a < 3; ++a)
-      for (int b = 0; b < 3; ++b) L[4 * a + b] = (a == b ? 1.f : 0.f) + s * K[3 * a + b] + (1.f - c) * K2[3 * a + b];
-    int p = par.p[j];
+    SmpltRod rod;
+    smplt_rodrigues(pose + 3 * j, rod, L);
+    const int p = par.p[j];
     for (int a = 0; a < 3; ++a) L[4 * a + 3] = J[3 * j + a] - (j > 0 ? J[3 * p + a] : 0.f);   // rel_joints (:479-480)
     L[12] = L[13] = L[14] = 0.f; L[15] = 1.f;
-    if (j == 0) {
-      for (int k = 0; k < 16; ++k) G[0][k] = L[k];
-    } else {                                                                       // sequential chain (:487-493)
-      for (int a = 0; a < 4; ++a)
-        for (int b = 0; b < 4; ++b) {
-          float acc = 0.f;
-          for (int k = 0; k < 4; ++k) acc = fmaf(G[p][4 * a + k], L[4 * k + b], acc);
-          G[j][4 * a + b] = acc;
-        }
-    }
+    if (j == 0) for (int k = 0; k < 16; ++k) G[0][k] = L[k];
+    else smplt_mm4(G[p], L, G[j]);                                                 // sequential chain (:487-493)
   }
   for (int j = 0; j < nj; ++j) {                                                   // A = G - [0 | G.[J;0]] (:500-503)
     for (int k = 0; k < 16; ++k) A[16 * j + k] = G[j][k];
@@ -88,7 +67,7 @@ __global__ void k_smpl_chain(const float* __restrict__ pose, const float* __rest
 __global__ void k_smpl_blend(const float* __restrict__ W, const float* __restrict__ A, const float* __restrict__ v_shaped,
                              const float* __restrict__ J, int nv, int nj, int concat, float* __restrict__ T,
                              float* __restrict__ verts) {
-  __shared__ float sA[SMPL_MAX_J * 16];
+  __shared__ float sA[SMPLT_MAX_J * 16];
   for (int k = threadIdx.x; k < nj * 16; k += blockDim.x) sA[k] = A[k];
   __syncthreads();
   int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -120,7 +99,7 @@ static int smpl_lbs(nm_ctx* ctx, const nm_smpl_model* m, const float* pose_dev, 
   NM_CHECK_LAUNCH(ctx);
   k_smpl_joints<<<nj * 3, 256, 0, st>>>(m->J_regressor, v_shaped, nv, J);
   NM_CHECK_LAUNCH(ctx);
-  SmplParents par;
+  SmpltParents par;
   for (int j = 0; j < nj; ++j) par.p[j] = m->parents[j];
   k_smpl_chain<<<1, 32, 0, st>>>(pose_dev, J, par, nj, A);
   NM_CHECK_LAUNCH(ctx);
@@ -132,7 +111,7 @@ static int smpl_lbs(nm_ctx* ctx, const nm_smpl_model* m, const float* pose_dev, 
 
 static int check_model(nm_ctx* ctx, const nm_smpl_model* m) {
   if (!m || !m->v_template || !m->shapedirs || !m->J_regressor || !m->weights || !m->parents || m->n_verts <= 0 ||
-      m->n_joints <= 0 || m->n_joints > SMPL_MAX_J || m->n_betas <= 0)
+      m->n_joints <= 0 || m->n_joints > SMPLT_MAX_J || m->n_betas <= 0)
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_smpl: bad model");
   return NM_OK;
 }
@@ -155,25 +134,6 @@ extern "C" int nm_smpl_vertex_transforms(nm_ctx* ctx, const nm_smpl_model* m, co
 }
 
 // --------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool inv4d(const double* m, double* o) {
-  double s0 = m[0] * m[5] - m[4] * m[1], s1 = m[0] * m[6] - m[4] * m[2], s2 = m[0] * m[7] - m[4] * m[3];
-  double s3 = m[1] * m[6] - m[5] * m[2], s4 = m[1] * m[7] - m[5] * m[3], s5 = m[2] * m[7] - m[6] * m[3];
-  double c5 = m[10] * m[15] - m[14] * m[11], c4 = m[9] * m[15] - m[13] * m[11], c3 = m[9] * m[14] - m[13] * m[10];
-  double c2 = m[8] * m[15] - m[12] * m[11], c1 = m[8] * m[14] - m[12] * m[10], c0 = m[8] * m[13] - m[12] * m[9];
-  double det = s0 * c5 - s1 * c4 + s2 * c3 + s3 * c2 - s4 * c1 + s5 * c0;
-  if (det == 0.0) return false;
-  double id = 1.0 / det;
-  o[0] = (m[5] * c5 - m[6] * c4 + m[7] * c3) * id;   o[1] = (-m[1] * c5 + m[2] * c4 - m[3] * c3) * id;
-  o[2] = (m[13] * s5 - m[14] * s4 + m[15] * s3) * id; o[3] = (-m[9] * s5 + m[10] * s4 - m[11] * s3) * id;
-  o[4] = (-m[4] * c5 + m[6] * c2 - m[7] * c1) * id;  o[5] = (m[0] * c5 - m[2] * c2 + m[3] * c1) * id;
-  o[6] = (-m[12] * s5 + m[14] * s2 - m[15] * s1) * id; o[7] = (m[8] * s5 - m[10] * s2 + m[11] * s1) * id;
-  o[8] = (m[4] * c4 - m[5] * c2 + m[7] * c0) * id;   o[9] = (-m[0] * c4 + m[1] * c2 - m[3] * c0) * id;
-  o[10] = (m[12] * s4 - m[13] * s2 + m[15] * s0) * id; o[11] = (-m[8] * s4 + m[9] * s2 - m[11] * s0) * id;
-  o[12] = (-m[4] * c3 + m[5] * c1 - m[6] * c0) * id; o[13] = (m[0] * c3 - m[1] * c1 + m[2] * c0) * id;
-  o[14] = (-m[12] * s3 + m[13] * s1 - m[14] * s0) * id; o[15] = (m[8] * s3 - m[9] * s1 + m[10] * s0) * id;
-  return true;
-}
-
 struct Mat4d { double v[16]; };
 
 // T_da2scene = S . align^T . T_t2pose . inv(T_t2da); world = T_da2scene . [da_vert;1]   (neuman_helper.py:316-326)
@@ -184,7 +144,7 @@ __global__ void k_smpl_scene(const float* __restrict__ T_pose, const float* __re
   if (v >= total) return;
   double P[16], D[16], Di[16], M[16], R[16];
   for (int k = 0; k < 16; ++k) { P[k] = (double)T_pose[(size_t)16 * v + k]; D[k] = (double)T_da[(size_t)16 * v + k]; }
-  inv4d(D, Di);
+  wd_inv4(D, Di);
   for (int a = 0; a < 4; ++a)
     for (int b = 0; b < 4; ++b) {
       double acc = 0.0;
@@ -305,7 +265,6 @@ extern "C" int nm_smpl_scene_backward(nm_ctx* ctx, const nm_smpl_model* m, const
   if (rc) return rc;
   if (!pose || !da_pose || !betas || !alignment || (!g_T && !g_world) || !g_pose || !g_betas || !g_alignment)
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_smpl_scene_backward: null argument");
-  if (m->n_joints > SMPLT_MAX_J) NM_FAIL(ctx, NM_ERR_INVALID, "nm_smpl_scene_backward: too many joints");
   cudaStream_t st = (cudaStream_t)stream;
   const int nv = m->n_verts, nj = m->n_joints, nb = m->n_betas;
   SmplTrainWs w{};

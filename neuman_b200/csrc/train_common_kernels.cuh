@@ -1,5 +1,5 @@
 // Shared by human_train_kernels.cuh and smpl_train_kernels.cuh: the build macros of the restricted CUDA subset (see
-// human_train_kernels.cuh) and the 4x4 inverse.
+// human_train_kernels.cuh) and the 4x4 inverse, which warp.cu and smpl.cu use as well.
 #pragma once
 #ifndef NM_EMU
 #define NM_KERNEL static __global__

@@ -18,9 +18,9 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <float.h>
 #include <math.h>
-#include <stdlib.h>
 
 #include "nm_internal.cuh"
+#include "train_common_kernels.cuh"
 
 // ---------------------------------------------------------------------------------------------
 // LBVH build
@@ -179,34 +179,6 @@ __device__ __forceinline__ V3<T> closest_on_tri(V3<T> p, V3<T> a, V3<T> b, V3<T>
   return madd(madd(a, ab, vb * den), ac, vc * den);
 }
 
-// 4x4 inverse (general, cofactor expansion) in double; returns false if singular
-__host__ __device__ __forceinline__ bool inv4(const double* m, double* o) {
-  double s0 = m[0] * m[5] - m[4] * m[1], s1 = m[0] * m[6] - m[4] * m[2], s2 = m[0] * m[7] - m[4] * m[3];
-  double s3 = m[1] * m[6] - m[5] * m[2], s4 = m[1] * m[7] - m[5] * m[3], s5 = m[2] * m[7] - m[6] * m[3];
-  double c5 = m[10] * m[15] - m[14] * m[11], c4 = m[9] * m[15] - m[13] * m[11], c3 = m[9] * m[14] - m[13] * m[10];
-  double c2 = m[8] * m[15] - m[12] * m[11], c1 = m[8] * m[14] - m[12] * m[10], c0 = m[8] * m[13] - m[12] * m[9];
-  double det = s0 * c5 - s1 * c4 + s2 * c3 + s3 * c2 - s4 * c1 + s5 * c0;
-  if (det == 0.0) return false;
-  double id = 1.0 / det;
-  o[0] = (m[5] * c5 - m[6] * c4 + m[7] * c3) * id;
-  o[1] = (-m[1] * c5 + m[2] * c4 - m[3] * c3) * id;
-  o[2] = (m[13] * s5 - m[14] * s4 + m[15] * s3) * id;
-  o[3] = (-m[9] * s5 + m[10] * s4 - m[11] * s3) * id;
-  o[4] = (-m[4] * c5 + m[6] * c2 - m[7] * c1) * id;
-  o[5] = (m[0] * c5 - m[2] * c2 + m[3] * c1) * id;
-  o[6] = (-m[12] * s5 + m[14] * s2 - m[15] * s1) * id;
-  o[7] = (m[8] * s5 - m[10] * s2 + m[11] * s1) * id;
-  o[8] = (m[4] * c4 - m[5] * c2 + m[7] * c0) * id;
-  o[9] = (-m[0] * c4 + m[1] * c2 - m[3] * c0) * id;
-  o[10] = (m[12] * s4 - m[13] * s2 + m[15] * s0) * id;
-  o[11] = (-m[8] * s4 + m[9] * s2 - m[11] * s0) * id;
-  o[12] = (-m[4] * c3 + m[5] * c1 - m[6] * c0) * id;
-  o[13] = (m[0] * c3 - m[1] * c1 + m[2] * c0) * id;
-  o[14] = (-m[12] * s3 + m[13] * s1 - m[14] * s0) * id;
-  o[15] = (m[8] * s3 - m[9] * s1 + m[10] * s0) * id;
-  return true;
-}
-
 __device__ __forceinline__ float box_d2(const BvhView& B, int node, V3<float> p) {
   const float4 l = __ldg(B.lo + node), h = __ldg(B.hi + node);
   float dx = fmaxf(fmaxf(l.x - p.x, p.x - h.x), 0.f), dy = fmaxf(fmaxf(l.y - p.y, p.y - h.y), 0.f),
@@ -321,7 +293,7 @@ __global__ void __launch_bounds__(128) k_warp_points(const float* __restrict__ v
   const double* Tc = T + 16 * (size_t)i2;
 #pragma unroll
   for (int k = 0; k < 16; ++k) M[k] = Ta[k] * la + Tb[k] * lb + Tc[k] * lc;          // (:56)
-  inv4(M, Mi);                                                                      // (:57)
+  wd_inv4(M, Mi);                                                                   // (:57)
   double cx = Mi[0] * P.x + Mi[1] * P.y + Mi[2] * P.z + Mi[3];                       // (:58)
   double cy = Mi[4] * P.x + Mi[5] * P.y + Mi[6] * P.z + Mi[7];
   double cz = Mi[8] * P.x + Mi[9] * P.y + Mi[10] * P.z + Mi[11];
@@ -347,17 +319,7 @@ __global__ void __launch_bounds__(256) k_warp_dirs(const double* __restrict__ ca
 }
 
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-static int ensure(nm_ctx* ctx, T** p, size_t* cap, size_t need) {
-  if (need <= *cap && *p) return NM_OK;
-  if (*p) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(*p)); *p = nullptr; }
-  size_t want = need + (need >> 2) + 16;
-  NM_CHECK_CUDA(ctx, cudaMalloc(p, want * sizeof(T)));
-  *cap = want;
-  return NM_OK;
-}
-
-// one device allocation per mesh holds the whole BVH (+ sort buffers); `cell_start` is its base pointer
+// one device allocation per mesh holds the whole BVH (+ sort buffers): NmMesh::bvh
 struct BvhLayout {
   size_t keys_in, keys_out, lo, hi, children, parent, visit, leaf_face, tri9, cub_tmp, box, total;
 };
@@ -384,7 +346,7 @@ static BvhView bvh_view(const NmMesh& m) {
   size_t cub_bytes = 0;
   cub::DeviceRadixSort::SortKeys(nullptr, cub_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, m.n_faces);
   BvhLayout L = bvh_layout(m.n_faces, cub_bytes);
-  char* base = reinterpret_cast<char*>(m.cell_start);
+  const char* base = m.bvh;
   BvhView B;
   B.n = m.n_faces;
   B.lo = reinterpret_cast<const float4*>(base + L.lo);
@@ -440,12 +402,8 @@ extern "C" int nm_mesh_set(nm_ctx* ctx, int actor, const float* verts, int32_t n
   size_t cub_bytes = 0;
   cub::DeviceRadixSort::SortKeys(nullptr, cub_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, n_faces);
   BvhLayout L = bvh_layout(n_faces, cub_bytes);
-  {
-    size_t cap = m.cap_cells;                 // capacity of the BVH block, in int32 units
-    if ((rc = ensure(ctx, &m.cell_start, &cap, L.total / sizeof(int32_t) + 1))) return rc;
-    m.cap_cells = cap;
-  }
-  char* base = reinterpret_cast<char*>(m.cell_start);
+  if ((rc = ensure(ctx, &m.bvh, &m.cap_bvh, L.total))) return rc;
+  char* base = m.bvh;
   auto* keys_in = reinterpret_cast<unsigned long long*>(base + L.keys_in);
   auto* keys_out = reinterpret_cast<unsigned long long*>(base + L.keys_out);
   float* tri9 = reinterpret_cast<float*>(base + L.tri9);
@@ -486,28 +444,18 @@ extern "C" int nm_warp_to_canonical(nm_ctx* ctx, int actor, const float* pts, in
   NmMesh& m = ctx->meshes[actor];
   long long n = (long long)R * S;
   // float64 canonical points: private scratch sized on demand (the frame drivers own ctx->ws)
-  if ((size_t)n * 3 > ctx->can64_cap) {
-    if (ctx->can64) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(ctx->can64)); ctx->can64 = nullptr; }
-    size_t want = (size_t)n * 3 + ((size_t)n * 3 >> 3);
-    NM_CHECK_CUDA(ctx, cudaMalloc(&ctx->can64, want * sizeof(double)));
-    ctx->can64_cap = want;
-  }
+  int rc;
+  if ((rc = ensure(ctx, &ctx->can64, &ctx->can64_cap, (size_t)n * 3))) return rc;
   double* can64 = ctx->can64;
   BvhView B = bvh_view(m);
-  // winning faces: the caller's buffer, or the tail of the float64 scratch (3 doubles per point, the ints take a sixth)
+  // winning faces: the caller's buffer, or a private scratch
   int32_t* fid = face_id;
   if (!fid) {
-    if ((size_t)n > ctx->face_cap) {
-      if (ctx->face_tmp) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(ctx->face_tmp)); ctx->face_tmp = nullptr; }
-      size_t want = (size_t)n + ((size_t)n >> 3);
-      NM_CHECK_CUDA(ctx, cudaMalloc(&ctx->face_tmp, want * sizeof(int32_t)));
-      ctx->face_cap = want;
-    }
+    if ((rc = ensure(ctx, &ctx->face_tmp, &ctx->face_cap, (size_t)n))) return rc;
     fid = ctx->face_tmp;
   }
   {
-    static const int lg_env = [] { const char* e = getenv("NEUMAN_WARP_PACKET"); return e ? atoi(e) : -1; }();
-    int lg = (lg_env >= 0 && lg_env <= 3) ? lg_env : 1;   // default: 2 rays x 16 samples
+    int lg = 1;                                           // packets of 2 rays x 16 samples, narrower where S or R need it
     while (lg > 0 && (S % (32 >> lg) != 0 || R < (1 << lg))) --lg;
     long long warps = lg == 0 ? (n + 31) / 32 : ((R + (1 << lg) - 1) >> lg) * (long long)(S / (32 >> lg));
     k_warp_nearest<<<(unsigned)((warps + 3) / 4), 128, 0, st>>>(B, pts, (long long)R, (int)S, lg, fid);
@@ -654,12 +602,8 @@ extern "C" int nm_signed_distance(nm_ctx* ctx, int actor, const float* pts, int6
   // winning faces: the caller's buffer, or a private scratch
   int32_t* fid = I;
   if (!fid) {
-    if ((size_t)n > ctx->face_cap) {
-      if (ctx->face_tmp) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(ctx->face_tmp)); ctx->face_tmp = nullptr; }
-      size_t want = (size_t)n + ((size_t)n >> 3);
-      NM_CHECK_CUDA(ctx, cudaMalloc(&ctx->face_tmp, want * sizeof(int32_t)));
-      ctx->face_cap = want;
-    }
+    int rc = ensure(ctx, &ctx->face_tmp, &ctx->face_cap, (size_t)n);
+    if (rc != NM_OK) return rc;
     fid = ctx->face_tmp;
   }
   const long long warps = (n + 31) / 32;

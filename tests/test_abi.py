@@ -55,3 +55,17 @@ def test_product_does_not_import_oracle():
             if fn.endswith((".py", ".cu", ".cuh", ".h")):
                 txt = open(os.path.join(dirpath, fn)).read()
                 assert "import oracle" not in txt and "from oracle" not in txt, fn
+
+
+def test_product_reads_only_known_environment_variables():
+    """No code path of the product is picked by an environment variable.  The ones it reads: the fp32 CUDA-core MLP
+    mode (NEUMAN_MLP_MODE, a supported mode), the policy for range errors (NEUMAN_RANGE_POLICY, reports, selects no
+    code) and the compiler the build uses (NVCC).  A read whose variable name is not a literal counts as unknown."""
+    allowed = {"NEUMAN_MLP_MODE", "NEUMAN_RANGE_POLICY", "NVCC"}
+    read = re.compile(r"""(?:getenv\(|os\.environ(?:\.get\(|\[)?)\s*(?:["']([A-Za-z0-9_]*)["'])?""")
+    pkg = os.path.join(ROOT, "neuman_b200")
+    csrc = os.path.join(pkg, "csrc")
+    files = [os.path.join(csrc, f) for f in os.listdir(csrc)] + [os.path.join(pkg, f) for f in os.listdir(pkg) if f.endswith(".py")]
+    found = [(os.path.basename(f), m.group(1)) for f in sorted(files) for m in read.finditer(open(f).read())]
+    assert {name for _, name in found} >= {"NEUMAN_MLP_MODE", "NEUMAN_RANGE_POLICY"}, found      # the scan sees the known reads
+    assert [(f, name) for f, name in found if name not in allowed] == []

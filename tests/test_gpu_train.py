@@ -176,8 +176,9 @@ def test_joiner_backward(kind, n, monkeypatch):
     g = torch.randn(n, 4)
 
     def product(torch_chain):
-        monkeypatch.setenv("NEUMAN_BWD_TORCH", "1" if torch_chain else "0")
-        monkeypatch.setenv("NEUMAN_DW_TORCH", "1" if torch_chain else "0")
+        if torch_chain:
+            monkeypatch.setattr(nag, "_chain_kernel", util.chain_torch)
+            monkeypatch.setattr(nag, "_dw_kernel", util.dw_torch)
         j.zero_grad()
         raw = j(pts.to(DEV), views.to(DEV))
         assert raw.requires_grad
