@@ -77,8 +77,11 @@ def train_batch(coarse_net, fine_net, optimizer, batch, opt, iteration=0, nan_gu
 
     The reference skips the backward pass when the loss is NaN (:214-218).  Here the backward is an fp16-operand chain
     with one power-of-two loss scale, so an overflow can also show up in the gradients only.  nan_guard:
-      'device' (default) -- no host sync: if the loss or any gradient is non-finite every gradient of the step is
-                            replaced by zero on the device before optimizer.step();
+      'device' (default) -- no host sync: if the loss or any gradient is non-finite the step is skipped on the device:
+                            the gradients are zeroed, and the parameters and every optimizer state tensor on their device
+                            (Adam's moments) are put back to their values before optimizer.step(), which would otherwise
+                            still move them by the momentum.  A step counter the optimizer keeps on the host (torch's
+                            non-capturable Adam) still counts the skipped step: reading the flag there is what 'host' does;
       'host'             -- the reference's behaviour: read the loss on the host, zero_grad() and skip backward on NaN;
       None               -- no guard."""
     optimizer.zero_grad()
@@ -96,12 +99,24 @@ def train_batch(coarse_net, fine_net, optimizer, batch, opt, iteration=0, nan_gu
         return total.detach()
     total.backward()
     if nan_guard == 'device':
-        grads = [p.grad for g in optimizer.param_groups for p in g['params'] if p.grad is not None]
-        if grads:
+        params = [p for g in optimizer.param_groups for p in g['params'] if p.grad is not None]
+        if params:
+            grads = [p.grad for p in params]
             ok = torch.isfinite(total.detach()) & torch.isfinite(torch.stack(torch._foreach_norm(grads))).all()
-            bad = ~ok
             for g in grads:
-                g.masked_fill_(bad, 0.0)
+                g.masked_fill_(~ok, 0.0)
+            dev = params[0].device
+            kept = [p.data for p in params] + [t for p in params for t in optimizer.state.get(p, {}).values()
+                                               if isinstance(t, torch.Tensor) and t.device == dev and t.is_floating_point()]
+            saved = torch._foreach_mul(kept, 1.0)
+            optimizer.step()
+            # kept = kept * ok + saved * (1 - ok): exact for either value of the flag (the step ran on zero gradients,
+            # so nothing in kept is non-finite unless it already was)
+            okf = ok.float()
+            torch._foreach_mul_(kept, okf)
+            torch._foreach_mul_(saved, 1.0 - okf)
+            torch._foreach_add_(kept, saved)
+            return total.detach()
     optimizer.step()
     return total.detach()
 
