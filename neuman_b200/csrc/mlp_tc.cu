@@ -275,9 +275,18 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
     const bool track = (it % rperiod) == (P.range_phase % rperiod);
     // ---- encodings (Embedder.forward, models/vanilla.py:82-92): threads 0-63 position, 64-127 direction of row wtid % 64 ----
     {
+      // Ray / view row of sample row0 + r: one 64-bit division per tile, then a 32-bit one per thread.  A per-thread
+      // 64-bit division compiles to a call on a path that depends on the thread's operands; with such a call in the
+      // tile loop ptxas serialises every wgmma of the kernel (warning C7520; tests/test_tc_sass.py).
       const int r = wtid & 63;
+      const int group = P.in.group;
+      long long g0 = 0;
+      uint32_t g0r = 0;
+      if (group > 0) { g0 = tile * 128 / group; g0r = (uint32_t)(tile * 128 - g0 * group); }
+      const uint32_t off = wg * TC_WG_ROWS + r;            // row0 + r - tile * 128
+      const long long g = group > 0 ? g0 + (g0r + off) / (uint32_t)group : row0 + r;
       float p[3] = {0.f, 0.f, 0.f}, v[3] = {0.f, 0.f, 0.f};
-      if (row0 + r < P.in.n) nm_fetch_sample(P.in, row0 + r, p, v);
+      if (row0 + r < P.in.n) nm_fetch_sample_at(P.in, row0 + r, g, p, v);
       uint32_t e[32];
       if (wtid < 64) {
         encode_f16(P.pos_pe, p, e, 30);

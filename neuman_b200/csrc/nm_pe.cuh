@@ -20,22 +20,24 @@ struct NmPeSpec {
   const float* table;  // posenc: freqs[n_freqs]; rotate: bvals[3*n_freqs][3]
 };
 
-__device__ __forceinline__ void nm_fetch_sample(const NmMlpInput& in, long long i, float p[3], float v[3]) {
+// Sample i whose ray (rays mode) / view row (pts mode) is g: i / group, or i in pts mode when group <= 0.
+__device__ __forceinline__ void nm_fetch_sample_at(const NmMlpInput& in, long long i, long long g, float p[3], float v[3]) {
   if (in.pts) {
     p[0] = in.pts[3 * i]; p[1] = in.pts[3 * i + 1]; p[2] = in.pts[3 * i + 2];
-    long long vi = in.group > 0 ? i / in.group : i;
-    if (in.views) { v[0] = in.views[3 * vi]; v[1] = in.views[3 * vi + 1]; v[2] = in.views[3 * vi + 2]; }
+    if (in.views) { v[0] = in.views[3 * g]; v[1] = in.views[3 * g + 1]; v[2] = in.views[3 * g + 2]; }
     else { v[0] = v[1] = v[2] = 0.f; }
   } else {
-    long long r = i / in.group;
     float zz = in.z[i];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      float d = in.dirs[3 * r + c];
+      float d = in.dirs[3 * g + c];
       v[c] = d;
-      p[c] = __fadd_rn(in.origins[3 * r + c], __fmul_rn(d, zz));
+      p[c] = __fadd_rn(in.origins[3 * g + c], __fmul_rn(d, zz));
     }
   }
+}
+__device__ __forceinline__ void nm_fetch_sample(const NmMlpInput& in, long long i, float p[3], float v[3]) {
+  nm_fetch_sample_at(in, i, in.pts && in.group <= 0 ? i : i / in.group, p, v);
 }
 
 // Writes the 2 channels produced by the (q)-th sin/cos pair of the encoding of x; q in [0, 3*n_freqs).

@@ -1,0 +1,98 @@
+"""Bit-for-bit comparison of the tensor-core MLP forward between two builds of the library.
+
+    python tools/fwd_digest.py dump OUT.json [--root TREE]     # run TREE's library (default: this tree) on seeded inputs
+    python tools/fwd_digest.py compare A.json B.json           # exit 1 unless every output is bit-identical
+
+`dump` runs k_mlp_tc on seeded inputs and records a SHA-256 of every output buffer: the training forward's raw, activation
+stash (st_x, st_f, st_v) and sign words, and the inference raw in per-sample, per-ray-view and fused ray modes.  Sizes
+cover ragged tiles, several waves of the persistent grid and a frame-sized ray chunk.  Run it once from each build's
+tree (each loads its own libneuman_b200.so) and compare the two files."""
+import argparse
+import hashlib
+import json
+import os
+import sys
+
+
+def _digest(t):
+    return hashlib.sha256(t.contiguous().cpu().numpy().tobytes()).hexdigest()
+
+
+def dump(out, root):
+    sys.path.insert(0, root)
+    import torch
+    import neuman_b200 as nb
+    from neuman_b200 import _lib, ops
+    from neuman_b200.ops import _p
+    from oracle import scenes
+    assert os.path.dirname(os.path.abspath(_lib.LIB_PATH)).startswith(os.path.abspath(root)), _lib.LIB_PATH
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    coarse, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False), 1)
+    human, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False, posenc="rotate"), 2)
+    T = 128 * torch.cuda.get_device_properties(0).multi_processor_count
+    res = {"lib": _lib.LIB_PATH}
+    for name, j in (("coarse", coarse.to(dev)), ("human", human.to(dev))):
+        ctx = ops._ctx_for(torch.empty(1, device=dev))
+        slot = ops.net_slot(j, ctx)
+        for n in (1, 129, 4173, 3 * T - 5):
+            g = torch.Generator(device=dev).manual_seed(n)
+            pts = torch.randn(n, 3, device=dev, generator=g) * 1.5
+            views = torch.nn.functional.normalize(torch.randn(n, 3, device=dev, generator=g), dim=-1)
+            # training forward, per-sample views
+            raw = torch.empty(n, 4, device=dev)
+            sx = torch.empty(8, n, 256, device=dev, dtype=torch.float16)
+            sf = torch.empty(n, 256, device=dev, dtype=torch.float16)
+            sv = torch.empty(n, 128, device=dev, dtype=torch.float16)
+            sm = torch.empty(9, n, 8, device=dev, dtype=torch.int32)
+            ctx.check(ctx.lib.nm_mlp_forward_train(ctx.h, slot, _p(pts), _p(views), n, 0, _p(raw), _p(sx), _p(sf), _p(sv),
+                                                   _p(sm), ctx.stream()))
+            torch.cuda.synchronize()
+            for k, v in (("raw", raw), ("st_x", sx), ("st_f", sf), ("st_v", sv), ("st_m", sm)):
+                res[f"{name}/train/n={n}/{k}"] = _digest(v)
+            # inference, per-sample views and one view row per 7 samples (n rounded down to a multiple of 7)
+            for group in (0, 7):
+                m = n if group == 0 else n - n % group
+                if m == 0:
+                    continue
+                vrows = views if group == 0 else views[: m // group].contiguous()
+                raw = torch.empty(m, 4, device=dev)
+                ctx.check(ctx.lib.nm_mlp_forward(ctx.h, slot, _lib.NM_MLP_TC_F16, _p(pts), _p(vrows), m, group, _p(raw),
+                                                 ctx.stream()))
+                torch.cuda.synchronize()
+                res[f"{name}/infer/n={m}/group={group}/raw"] = _digest(raw)
+        # fused ray mode (pts = o + d z), up to a frame's chunk of 32768 rays x 256 samples
+        for R, S in ((1, 1), (33, 33), (97, 128), (4096, 128), (32768, 256)):
+            g = torch.Generator(device=dev).manual_seed(R * 1000 + S)
+            o = torch.randn(R, 3, device=dev, generator=g) * 0.3
+            d = torch.nn.functional.normalize(torch.randn(R, 3, device=dev, generator=g), dim=-1)
+            z = torch.sort(torch.rand(R, S, device=dev, generator=g) * 3.14, dim=-1)[0].contiguous()
+            raw = ops.mlp_forward_rays(j, o, d, z, mode=_lib.NM_MLP_TC_F16)
+            torch.cuda.synchronize()
+            res[f"{name}/rays/R={R}/S={S}/raw"] = _digest(raw)
+    _lib.Context.get(0).range_check()
+    with open(out, "w") as f:
+        json.dump(res, f, indent=1, sort_keys=True)
+    print(f"{len(res) - 1} digests of {res['lib']} -> {out}")
+
+
+def compare(a, b):
+    A, B = (json.load(open(p)) for p in (a, b))
+    keys = sorted((set(A) | set(B)) - {"lib"})
+    bad = [k for k in keys if A.get(k) != B.get(k)]
+    for k in bad:
+        print("DIFFERENT", k)
+    print(f"{len(keys) - len(bad)} of {len(keys)} outputs bit-identical ({A['lib']} vs {B['lib']})")
+    return 1 if bad else 0
+
+
+if __name__ == "__main__":
+    ap = argparse.ArgumentParser()
+    ap.add_argument("cmd", choices=["dump", "compare"])
+    ap.add_argument("files", nargs="+")
+    ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    a = ap.parse_args()
+    if a.cmd == "dump":
+        dump(a.files[0], os.path.abspath(a.root))
+    else:
+        sys.exit(compare(*a.files))
