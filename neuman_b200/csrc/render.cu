@@ -12,18 +12,6 @@
 
 namespace {
 
-struct Arena {
-  char* base = nullptr;
-  size_t off = 0, cap = 0;
-  template <typename T>
-  T* take(size_t n) {
-    off = (off + 255) & ~size_t(255);
-    T* p = reinterpret_cast<T*>(base + off);
-    off += n * sizeof(T);
-    return p;
-  }
-};
-
 // general torch.linspace(start, end, steps)[i] in float32 (see nm_linspace01)
 __device__ __forceinline__ float linspace_f(float start, float end, int i, int steps) {
   if (steps <= 1) return start;
@@ -78,11 +66,6 @@ __global__ void k_move_rows(const int32_t* __restrict__ idx, long long n, int wi
   else dst[t] = src[r * width + c];
 }
 
-__global__ void k_mark_rows(const int32_t* __restrict__ idx, long long n, float* __restrict__ flag) {
-  long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < n) flag[idx[t]] = 1.f;
-}
-
 // flag[r] = 1 for the rays of a near/far pair that hit (near < far)
 __global__ void k_mark_hits(const float* __restrict__ near_v, const float* __restrict__ far_v, long long R,
                             float* __restrict__ flag) {
@@ -110,18 +93,87 @@ __global__ void k_fill(float* __restrict__ p, long long n, float v) {
     if (_rc != NM_OK) return _rc; \
   } while (0)
 
-int check_common(nm_ctx* ctx, const nm_camera* cam, const nm_render_opts* opt, int64_t pix0, int64_t n, const int32_t* pixels,
-                 const char* who) {
+// Bump allocator over the drivers' workspace; every buffer starts on a 256-byte boundary.  With a zero base it
+// only measures: render_frame runs a driver's layout once that way to size the workspace.
+struct Arena {
+  uintptr_t base = 0;
+  size_t off = 0;
+  template <typename T>
+  T* take(size_t n) {
+    off = (off + 255) & ~size_t(255);
+    T* p = reinterpret_cast<T*>(base + off);
+    off += n * sizeof(T);
+    return p;
+  }
+};
+
+// Output planes of n rays: rgb [n,3], depth [n], acc [n].
+struct Planes {
+  float *rgb = nullptr, *depth = nullptr, *acc = nullptr;
+};
+
+int check_frame(nm_ctx* ctx, const nm_camera* cam, const nm_render_opts* opt, int64_t pix0, int64_t n,
+                const int32_t* pixels, const float* rgb, const char* who) {
   if (!cam || !opt || n < 0 || (!pixels && (pix0 < 0 || pix0 + n > (int64_t)cam->H * cam->W)))
     NM_FAIL(ctx, NM_ERR_INVALID, std::string(who) + ": bad camera/options/pixel range");
   if (opt->samples_per_ray <= 0 || opt->importance_samples_per_ray < 0)
     NM_FAIL(ctx, NM_ERR_INVALID, std::string(who) + ": bad sample counts");
+  if (!rgb) NM_FAIL(ctx, NM_ERR_INVALID, std::string(who) + ": null rgb");
   return NM_OK;
 }
 
-int chunk_of(const nm_render_opts* opt) { return opt->rays_per_batch > 0 ? opt->rays_per_batch : 32768; }
+int check_slot(nm_ctx* ctx, int slot, const char* who) {
+  if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !ctx->nets[slot].packed)
+    NM_FAIL(ctx, NM_ERR_STATE, std::string(who) + ": net slot not packed");
+  return NM_OK;
+}
 
-int slot_ok(nm_ctx* ctx, int slot) { return slot >= 0 && slot < NM_MAX_NET_SLOTS && ctx->nets[slot].packed; }
+int check_mesh(nm_ctx* ctx, int actor, const char* who) {
+  if (actor < 0 || actor >= NM_MAX_ACTORS || !ctx->meshes[actor].set)
+    NM_FAIL(ctx, NM_ERR_STATE, std::string(who) + ": mesh not set");
+  return NM_OK;
+}
+
+// The frame loop of every driver, over chunks of at most C rays.  layout(A, C) takes the driver's own buffers for such
+// a chunk; it runs once on a zero base to size the workspace and once on the workspace.  For each chunk the rays are
+// generated into o/d (ray_mode as in nm_raygen) and body(c, o, d, dst) runs on its c rays.  dst holds the chunk's
+// output planes: the caller's device buffers, or staging when the output goes to the host or the caller's plane is
+// null.  With host output the staged planes are copied back and the stream synchronised before the next chunk.
+template <typename Layout, typename Body>
+int render_frame(nm_ctx* ctx, const nm_camera* cam, const nm_render_opts* opt, int ray_mode, int64_t pix0, int64_t n,
+                 const int32_t* pixels, const Planes& out, int host_out, cudaStream_t st, Layout&& layout, Body&& body) {
+  const int64_t C = std::min<int64_t>(opt->rays_per_batch > 0 ? opt->rays_per_batch : 32768, n > 0 ? n : 1);
+  float *o, *d;
+  Planes stage;
+  auto take_all = [&](Arena& A) {
+    o = A.take<float>(3 * C); d = A.take<float>(3 * C);
+    stage.rgb = A.take<float>(3 * C); stage.depth = A.take<float>(C); stage.acc = A.take<float>(C);
+    layout(A, C);
+  };
+  Arena A;
+  take_all(A);
+  char* ws = nullptr;
+  TRY(nm_impl_workspace(ctx, A.off, &ws));
+  A = Arena{reinterpret_cast<uintptr_t>(ws)};
+  take_all(A);
+  ctx->last_mlp_evals = 0; ctx->last_hit_rays = 0;
+  for (int64_t i = 0; i < n; i += C) {
+    const int64_t c = std::min<int64_t>(C, n - i);
+    TRY(nm_impl_raygen(ctx, cam, ray_mode, pix0 + i, c, nullptr, pixels ? pixels + i : nullptr, o, d, st));
+    auto dst = [&](float* p, float* s, int w) { return host_out || !p ? s : p + w * i; };
+    TRY(body(c, o, d, Planes{dst(out.rgb, stage.rgb, 3), dst(out.depth, stage.depth, 1), dst(out.acc, stage.acc, 1)}));
+    if (host_out) {
+      auto back = [&](float* p, const float* s, int w) {
+        return p ? cudaMemcpyAsync(p + w * i, s, w * c * sizeof(float), cudaMemcpyDeviceToHost, st) : cudaSuccess;
+      };
+      NM_CHECK_CUDA(ctx, back(out.rgb, stage.rgb, 3));
+      NM_CHECK_CUDA(ctx, back(out.depth, stage.depth, 1));
+      NM_CHECK_CUDA(ctx, back(out.acc, stage.acc, 1));
+      NM_CHECK_CUDA(ctx, cudaStreamSynchronize(st));
+    }
+  }
+  return NM_OK;
+}
 
 // background coarse (+fine) pass over C rays already in o/d: leaves raw/z of the last pass in
 // (*raw_out, *z_out) with *S_out samples.  utils/render_utils.py:141-153 / :287-298 / :398-409
@@ -145,9 +197,68 @@ int bkg_pass(nm_ctx* ctx, int coarse, int fine, const nm_render_opts* opt, const
   return NM_OK;
 }
 
-int copy_out(nm_ctx* ctx, float* dst, const float* src, size_t n, int host_out, cudaStream_t st) {
-  if (!dst || dst == src) return NM_OK;
-  NM_CHECK_CUDA(ctx, cudaMemcpyAsync(dst, src, n * sizeof(float), host_out ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, st));
+// The rays the actors hit in one chunk: per actor, near/far against its set mesh and the indices of the rays with
+// near < far; with `uni` (multi-person) also the rays any actor hits.  Plus the human branch's scratch for them.
+struct Hits {
+  int n; bool uni; const int32_t* actors;   // actors, multi-person, their mesh slots
+  float *nr[NM_MAX_ACTORS], *fr[NM_MAX_ACTORS];
+  int32_t* idx[NM_MAX_ACTORS];
+  int64_t count[NM_MAX_ACTORS + 1];   // hit rays per actor, then of the union
+  int32_t* uidx = nullptr;
+  float *flag = nullptr, *zeros = nullptr;
+  float *oh, *dh, *nh, *fh, *pts, *cpts, *cdirs, *z, *raw;   // gathered rays, samples, canonical points, net output
+  float *rgb, *depth, *acc;                                  // their composite
+  void take(Arena& A, int64_t C, int S) {
+    for (int a = 0; a < n; ++a) { nr[a] = A.take<float>(C); fr[a] = A.take<float>(C); idx[a] = A.take<int32_t>(C); }
+    if (uni) { uidx = A.take<int32_t>(C); flag = A.take<float>(C); zeros = A.take<float>(C); }
+    oh = A.take<float>(3 * C); dh = A.take<float>(3 * C); nh = A.take<float>(C); fh = A.take<float>(C);
+    pts = A.take<float>(3 * C * S); cpts = A.take<float>(3 * C * S); cdirs = A.take<float>(3 * C * S);
+    z = A.take<float>(C * S); raw = A.take<float>(4 * C * S);
+    rgb = A.take<float>(3 * C); depth = A.take<float>(C); acc = A.take<float>(C);
+  }
+};
+
+// Queues the hit lists of the c rays in o/d (utils/render_utils.py:198-206 / :299 / :415) and the read-back of their
+// counts, whose arrival on the host ctx->ev_counts marks.  hit_counts() waits for them.
+int hit_lists(nm_ctx* ctx, Hits& h, float geo_threshold, const float* o, const float* d, int64_t c, cudaStream_t st) {
+  if (!ctx->ev_counts) NM_CHECK_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_counts, cudaEventDisableTiming));
+  NM_CHECK_CUDA(ctx, cudaMemsetAsync(ctx->d_counter, 0, sizeof(int32_t) * (h.n + 1), st));
+  if (h.uni) { LAUNCH1D(k_fill, c, st, h.flag, c, 0.f); LAUNCH1D(k_fill, c, st, h.zeros, c, 0.f); }
+  for (int a = 0; a < h.n; ++a) {
+    TRY(nm_impl_near_far_mesh(ctx, ctx->meshes[h.actors[a]], o, d, c, geo_threshold, h.nr[a], h.fr[a], st));
+    LAUNCH1D(k_compact_hits, c, st, h.nr[a], h.fr[a], c, h.idx[a], ctx->d_counter + a);
+    if (h.uni) LAUNCH1D(k_mark_hits, c, st, h.nr[a], h.fr[a], c, h.flag);
+  }
+  if (h.uni) LAUNCH1D(k_compact_hits, c, st, h.zeros, h.flag, c, h.uidx, ctx->d_counter + h.n);
+  NM_CHECK_CUDA(ctx, cudaMemcpyAsync(ctx->h_counter, ctx->d_counter, sizeof(int32_t) * (h.n + 1), cudaMemcpyDeviceToHost, st));
+  NM_CHECK_CUDA(ctx, cudaEventRecord(ctx->ev_counts, st));
+  return NM_OK;
+}
+
+// Waits for the counts of hit_lists() and adds the actors' hit rays to the frame's statistics (nm_last_render_stats).
+int hit_counts(nm_ctx* ctx, Hits& h) {
+  NM_CHECK_CUDA(ctx, cudaEventSynchronize(ctx->ev_counts));
+  for (int a = 0; a <= h.n; ++a) h.count[a] = ctx->h_counter[a];
+  for (int a = 0; a < h.n; ++a) ctx->last_hit_rays += h.count[a];
+  return NM_OK;
+}
+
+// human branch for the rays actor a hits in one chunk: gathers them from o/d into h.oh/dh/nh/fh, then samples, warp,
+// net.  Leaves h.raw [Rh,S,4] and h.z [Rh,S].
+int human_branch(nm_ctx* ctx, int slot, const nm_render_opts* opt, const float* o, const float* d, const Hits& h, int a,
+                 bool render_can, cudaStream_t st) {
+  const int S = opt->samples_per_ray;
+  const int64_t Rh = h.count[a];
+  LAUNCH1D(k_gather_rays, Rh, st, h.idx[a], (int)Rh, o, d, h.nr[a], h.fr[a], h.oh, h.dh, h.nh, h.fh);
+  if (render_can) {                                                          // (:214-216)
+    TRY(nm_ray_to_samples(ctx, h.oh, h.dh, h.nh, h.fh, 0, 0, Rh, S, 0, nullptr, nullptr, nullptr, h.z, st));
+    TRY(nm_mlp_forward_rays(ctx, slot, opt->mlp_mode, h.oh, h.dh, h.z, Rh, S, h.raw, st));
+  } else {
+    TRY(nm_ray_to_samples(ctx, h.oh, h.dh, h.nh, h.fh, 0, 0, Rh, S, 0, nullptr, h.pts, nullptr, h.z, st));
+    TRY(nm_warp_to_canonical(ctx, h.actors[a], h.pts, Rh, S, h.cpts, h.cdirs, nullptr, nullptr, st));   // (:218-225)
+    TRY(nm_mlp_forward(ctx, slot, opt->mlp_mode, h.cpts, h.cdirs, Rh * S, 0, h.raw, st));
+  }
+  ctx->last_mlp_evals += Rh * S;
   return NM_OK;
 }
 
@@ -158,125 +269,54 @@ extern "C" int nm_render_vanilla(nm_ctx* ctx, int coarse_slot, int fine_slot, co
                                  const nm_render_opts* opt, int64_t pix0, int64_t n, const int32_t* pixels, float* rgb,
                                  float* depth, int32_t host_out, void* stream) {
   NM_ENTER(ctx);
-  TRY(check_common(ctx, cam, opt, pix0, n, pixels, "nm_render_vanilla"));
-  if (!slot_ok(ctx, coarse_slot) || (fine_slot >= 0 && !slot_ok(ctx, fine_slot)))
-    NM_FAIL(ctx, NM_ERR_STATE, "nm_render_vanilla: net slot not packed");
-  if (!rgb) NM_FAIL(ctx, NM_ERR_INVALID, "nm_render_vanilla: null rgb");
+  TRY(check_frame(ctx, cam, opt, pix0, n, pixels, rgb, __func__));
+  TRY(check_slot(ctx, coarse_slot, __func__));
+  if (fine_slot >= 0) TRY(check_slot(ctx, fine_slot, __func__));
   cudaStream_t st = (cudaStream_t)stream;
   const int S = opt->samples_per_ray, N = fine_slot >= 0 ? opt->importance_samples_per_ray : 0;
-  const int64_t C = std::min<int64_t>(chunk_of(opt), n > 0 ? n : 1);
-  ctx->last_mlp_evals = 0; ctx->last_hit_rays = 0;
-  size_t bytes = (size_t)C * (6 + S + 4 * S + S + (S + N) + 4 * (S + N) + 4) * sizeof(float) + 16 * 256;
-  Arena A;
-  TRY(nm_impl_workspace(ctx, bytes, &A.base));
-  float* o = A.take<float>(3 * C); float* d = A.take<float>(3 * C);
-  float* z_c = A.take<float>(C * S); float* raw_c = A.take<float>(4 * C * S); float* w_c = A.take<float>(C * S);
-  float* z_f = A.take<float>(C * (S + N)); float* raw_f = A.take<float>(4 * C * (S + N));
-  float* rgb_s = A.take<float>(3 * C); float* dep_s = A.take<float>(C);
-  if (A.off > ctx->ws_bytes) NM_FAIL(ctx, NM_ERR_STATE, "render: workspace arena overflow (internal sizing bug)");
-  for (int64_t i = 0; i < n; i += C) {
-    int64_t c = std::min<int64_t>(C, n - i);
-    TRY(nm_impl_raygen(ctx, cam, 1, pix0 + i, c, nullptr, pixels ? pixels + i : nullptr, o, d, st));                       // shot_all_rays (:122)
-    float *raw, *z; int St;
-    TRY(bkg_pass(ctx, coarse_slot, fine_slot, opt, o, d, c, z_c, raw_c, w_c, z_f, raw_f, &raw, &z, &St, st));
-    float* rgb_dst = host_out ? rgb_s : rgb + 3 * i;
-    float* dep_dst = host_out ? dep_s : (depth ? depth + i : nullptr);
-    TRY(nm_raw2outputs(ctx, raw, z, d, c, St, nullptr, 1.f, opt->white_bkg, rgb_dst, nullptr, nullptr, nullptr, dep_dst, st));
-    if (host_out) {
-      TRY(copy_out(ctx, rgb + 3 * i, rgb_s, 3 * c, 1, st));
-      if (depth) TRY(copy_out(ctx, depth + i, dep_s, c, 1, st));
-      NM_CHECK_CUDA(ctx, cudaStreamSynchronize(st));   // staging buffers are reused by the next chunk
-    }
-  }
-  return NM_OK;
+  float *z_c, *raw_c, *w_c, *z_f, *raw_f;
+  return render_frame(ctx, cam, opt, 1, pix0, n, pixels, Planes{rgb, depth, nullptr}, host_out, st,   // shot_all_rays (:122)
+    [&](Arena& A, int64_t C) {
+      z_c = A.take<float>(C * S); raw_c = A.take<float>(4 * C * S); w_c = A.take<float>(C * S);
+      z_f = A.take<float>(C * (S + N)); raw_f = A.take<float>(4 * C * (S + N));
+    },
+    [&](int64_t c, const float* o, const float* d, const Planes& dst) -> int {
+      float *raw, *z; int St;
+      TRY(bkg_pass(ctx, coarse_slot, fine_slot, opt, o, d, c, z_c, raw_c, w_c, z_f, raw_f, &raw, &z, &St, st));
+      return nm_raw2outputs(ctx, raw, z, d, c, St, nullptr, 1.f, opt->white_bkg, dst.rgb, nullptr, nullptr, nullptr, dst.depth, st);
+    });
 }
 
 // ---------------------------------------------------------------------------------------------
-// human branch for the hit rays of one chunk: samples, warp, net, (optional) own composite.
-// Produces raw_h [Rh,S,4], z_h [Rh,S] for the compacted hit rays.
-static int human_branch(nm_ctx* ctx, int slot, int actor, const nm_render_opts* opt, const float* oh, const float* dh,
-                        const float* nh, const float* fh, int64_t Rh, float* pts, float* can_pts, float* can_dirs,
-                        float* z_h, float* raw_h, bool render_can, cudaStream_t st) {
-  const int S = opt->samples_per_ray;
-  if (render_can) {                                                          // (:214-216)
-    TRY(nm_ray_to_samples(ctx, oh, dh, nh, fh, 0, 0, Rh, S, 0, nullptr, nullptr, nullptr, z_h, st));
-    TRY(nm_mlp_forward_rays(ctx, slot, opt->mlp_mode, oh, dh, z_h, Rh, S, raw_h, st));
-  } else {
-    TRY(nm_ray_to_samples(ctx, oh, dh, nh, fh, 0, 0, Rh, S, 0, nullptr, pts, nullptr, z_h, st));
-    TRY(nm_warp_to_canonical(ctx, actor, pts, Rh, S, can_pts, can_dirs, nullptr, nullptr, st));   // (:218-225)
-    TRY(nm_mlp_forward(ctx, slot, opt->mlp_mode, can_pts, can_dirs, Rh * S, 0, raw_h, st));
-  }
-  ctx->last_mlp_evals += Rh * S;
-  return NM_OK;
-}
-
-static int compact(nm_ctx* ctx, const float* near_v, const float* far_v, int64_t c, int32_t* hit_idx, int64_t* Rh,
-                   cudaStream_t st) {
-  NM_CHECK_CUDA(ctx, cudaMemsetAsync(ctx->d_counter, 0, sizeof(int32_t), st));
-  k_compact_hits<<<(unsigned)((c + 255) / 256), 256, 0, st>>>(near_v, far_v, c, hit_idx, ctx->d_counter);
-  NM_CHECK_LAUNCH(ctx);
-  NM_CHECK_CUDA(ctx, cudaMemcpyAsync(ctx->h_counter, ctx->d_counter, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  NM_CHECK_CUDA(ctx, cudaStreamSynchronize(st));
-  *Rh = ctx->h_counter[0];
-  return NM_OK;
-}
-
 extern "C" int nm_render_smpl_nerf(nm_ctx* ctx, int human_slot, int actor, const nm_camera* cam,
                                    const nm_render_opts* opt, int64_t pix0, int64_t n, const int32_t* pixels, float* rgb,
                                    float* depth, float* acc, int32_t host_out, void* stream) {
   NM_ENTER(ctx);
-  TRY(check_common(ctx, cam, opt, pix0, n, pixels, "nm_render_smpl_nerf"));
-  if (!slot_ok(ctx, human_slot)) NM_FAIL(ctx, NM_ERR_STATE, "nm_render_smpl_nerf: net slot not packed");
-  if (actor < 0 || actor >= NM_MAX_ACTORS || !ctx->meshes[actor].set)
-    NM_FAIL(ctx, NM_ERR_STATE, "nm_render_smpl_nerf: mesh not set");
-  if (!rgb) NM_FAIL(ctx, NM_ERR_INVALID, "nm_render_smpl_nerf: null rgb");
+  TRY(check_frame(ctx, cam, opt, pix0, n, pixels, rgb, __func__));
+  TRY(check_slot(ctx, human_slot, __func__));
+  TRY(check_mesh(ctx, actor, __func__));
   cudaStream_t st = (cudaStream_t)stream;
   const int S = opt->samples_per_ray;
-  const int64_t C = std::min<int64_t>(chunk_of(opt), n > 0 ? n : 1);
-  ctx->last_mlp_evals = 0; ctx->last_hit_rays = 0;
-  size_t bytes = (size_t)C * (6 + 2 + 1 + 8 + 9 * S + S + 4 * S + 5 + 5) * sizeof(float) + 32 * 256;
-  Arena A;
-  TRY(nm_impl_workspace(ctx, bytes, &A.base));
-  float* o = A.take<float>(3 * C); float* d = A.take<float>(3 * C);
-  float* nr = A.take<float>(C); float* fr = A.take<float>(C);
-  int32_t* hit = A.take<int32_t>(C);
-  float* oh = A.take<float>(3 * C); float* dh = A.take<float>(3 * C); float* nh = A.take<float>(C); float* fh = A.take<float>(C);
-  float* pts = A.take<float>(3 * C * S); float* cpts = A.take<float>(3 * C * S); float* cdirs = A.take<float>(3 * C * S);
-  float* z_h = A.take<float>(C * S); float* raw_h = A.take<float>(4 * C * S);
-  float* rgb_h = A.take<float>(3 * C); float* dep_h = A.take<float>(C); float* acc_h = A.take<float>(C);
-  float* rgb_s = A.take<float>(3 * C); float* dep_s = A.take<float>(C); float* acc_s = A.take<float>(C);
-  const NmMesh& mesh = ctx->meshes[actor];
-  if (A.off > ctx->ws_bytes) NM_FAIL(ctx, NM_ERR_STATE, "render: workspace arena overflow (internal sizing bug)");
-  for (int64_t i = 0; i < n; i += C) {
-    int64_t c = std::min<int64_t>(C, n - i);
-    TRY(nm_impl_raygen(ctx, cam, 0, pix0 + i, c, nullptr, pixels ? pixels + i : nullptr, o, d, st));                        // shot_rays (:186)
-    TRY(nm_impl_near_far_mesh(ctx, mesh, o, d, c, opt->geo_threshold, nr, fr, st));   // (:198)
-    int64_t Rh = 0;
-    TRY(compact(ctx, nr, fr, c, hit, &Rh, st));
-    ctx->last_hit_rays += Rh;
-    float* rgb_dst = host_out ? rgb_s : rgb + 3 * i;
-    float* dep_dst = host_out ? dep_s : (depth ? depth + i : dep_s);
-    float* acc_dst = host_out ? acc_s : (acc ? acc + i : acc_s);
-    LAUNCH1D(k_fill, 3 * c, st, rgb_dst, 3 * c, opt->white_bkg ? 1.f : 0.f);             // miss rays (:199-205)
-    LAUNCH1D(k_fill, c, st, dep_dst, c, 0.f);
-    LAUNCH1D(k_fill, c, st, acc_dst, c, 0.f);
-    if (Rh > 0) {
-      LAUNCH1D(k_gather_rays, Rh, st, hit, (int)Rh, o, d, nr, fr, oh, dh, nh, fh);
-      TRY(human_branch(ctx, human_slot, actor, opt, oh, dh, nh, fh, Rh, pts, cpts, cdirs, z_h, raw_h, opt->render_can != 0, st));
-      TRY(nm_raw2outputs(ctx, raw_h, z_h, dh, Rh, S, nullptr, opt->interval_comp, opt->white_bkg, rgb_h, nullptr, acc_h,
-                         nullptr, dep_h, st));                                          // (:229-230)
-      LAUNCH1D(k_move_rows, Rh * 3, st, hit, Rh, 3, rgb_h, rgb_dst, 1);                  // (:231-233)
-      LAUNCH1D(k_move_rows, Rh, st, hit, Rh, 1, dep_h, dep_dst, 1);
-      LAUNCH1D(k_move_rows, Rh, st, hit, Rh, 1, acc_h, acc_dst, 1);
-    }
-    if (host_out) {
-      TRY(copy_out(ctx, rgb + 3 * i, rgb_s, 3 * c, 1, st));
-      if (depth) TRY(copy_out(ctx, depth + i, dep_s, c, 1, st));
-      if (acc) TRY(copy_out(ctx, acc + i, acc_s, c, 1, st));
-      NM_CHECK_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-  }
-  return NM_OK;
+  Hits h{1, false, &actor};
+  return render_frame(ctx, cam, opt, 0, pix0, n, pixels, Planes{rgb, depth, acc}, host_out, st,   // shot_rays (:186)
+    [&](Arena& A, int64_t C) { h.take(A, C, S); },
+    [&](int64_t c, const float* o, const float* d, const Planes& dst) -> int {
+      TRY(hit_lists(ctx, h, opt->geo_threshold, o, d, c, st));
+      TRY(hit_counts(ctx, h));
+      const int64_t Rh = h.count[0];
+      LAUNCH1D(k_fill, 3 * c, st, dst.rgb, 3 * c, opt->white_bkg ? 1.f : 0.f);             // miss rays (:199-205)
+      LAUNCH1D(k_fill, c, st, dst.depth, c, 0.f);
+      LAUNCH1D(k_fill, c, st, dst.acc, c, 0.f);
+      if (Rh > 0) {
+        TRY(human_branch(ctx, human_slot, opt, o, d, h, 0, opt->render_can != 0, st));
+        TRY(nm_raw2outputs(ctx, h.raw, h.z, h.dh, Rh, S, nullptr, opt->interval_comp, opt->white_bkg, h.rgb, nullptr, h.acc,
+                           nullptr, h.depth, st));                                          // (:229-230)
+        LAUNCH1D(k_move_rows, Rh * 3, st, h.idx[0], Rh, 3, h.rgb, dst.rgb, 1);             // (:231-233)
+        LAUNCH1D(k_move_rows, Rh, st, h.idx[0], Rh, 1, h.depth, dst.depth, 1);
+        LAUNCH1D(k_move_rows, Rh, st, h.idx[0], Rh, 1, h.acc, dst.acc, 1);
+      }
+      return NM_OK;
+    });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -285,143 +325,99 @@ extern "C" int nm_render_hybrid(nm_ctx* ctx, int coarse_slot, int fine_slot, int
                                 const nm_camera* cam, const nm_render_opts* opt, int64_t pix0, int64_t n,
                                 const int32_t* pixels, float* rgb, float* depth, float* acc, int32_t host_out, void* stream) {
   NM_ENTER(ctx);
-  TRY(check_common(ctx, cam, opt, pix0, n, pixels, "nm_render_hybrid"));
-  if (!slot_ok(ctx, coarse_slot) || (fine_slot >= 0 && !slot_ok(ctx, fine_slot)))
-    NM_FAIL(ctx, NM_ERR_STATE, "nm_render_hybrid: bkg net slot not packed");
+  TRY(check_frame(ctx, cam, opt, pix0, n, pixels, rgb, __func__));
+  TRY(check_slot(ctx, coarse_slot, __func__));
+  if (fine_slot >= 0) TRY(check_slot(ctx, fine_slot, __func__));
   if (n_actors < 1 || n_actors > NM_MAX_ACTORS || !human_slots || !actors || (!multi_person && n_actors != 1))
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_render_hybrid: bad actor list");
-  for (int a = 0; a < n_actors; ++a)
-    if (!slot_ok(ctx, human_slots[a]) || actors[a] < 0 || actors[a] >= NM_MAX_ACTORS || !ctx->meshes[actors[a]].set)
-      NM_FAIL(ctx, NM_ERR_STATE, "nm_render_hybrid: human net or mesh not set");
-  if (!rgb) NM_FAIL(ctx, NM_ERR_INVALID, "nm_render_hybrid: null rgb");
+  for (int a = 0; a < n_actors; ++a) {
+    TRY(check_slot(ctx, human_slots[a], __func__));
+    TRY(check_mesh(ctx, actors[a], __func__));
+  }
   cudaStream_t st = (cudaStream_t)stream;
   const int S = opt->samples_per_ray, N = fine_slot >= 0 ? opt->importance_samples_per_ray : 0;
-  const int Sb = S + N;
-  const int n_lists = 1 + n_actors;
-  const int Sm = Sb + n_actors * S;
-  const int64_t C = std::min<int64_t>(chunk_of(opt), n > 0 ? n : 1);
-  ctx->last_mlp_evals = 0; ctx->last_hit_rays = 0;
-  size_t per_ray = 6 + 2 + 1 + 8 + 9 * S + (size_t)5 * S + 6 * S + 5 * Sb + 5 * Sb + 5 * Sm + 8 + 5 + 3 * (size_t)n_actors +
-                   (multi_person ? (size_t)10 * S * n_actors + 2 : 0);
-  size_t bytes = (size_t)C * per_ray * sizeof(float) + 96 * 256;
-  Arena A;
-  TRY(nm_impl_workspace(ctx, bytes, &A.base));
-  float* o = A.take<float>(3 * C); float* d = A.take<float>(3 * C);
-  float* nr_a[NM_MAX_ACTORS]; float* fr_a[NM_MAX_ACTORS]; int32_t* hit_a[NM_MAX_ACTORS];
-  for (int a = 0; a < n_actors; ++a) { nr_a[a] = A.take<float>(C); fr_a[a] = A.take<float>(C); hit_a[a] = A.take<int32_t>(C); }
-  int32_t* hit = A.take<int32_t>(C);                                                // rays any actor hits (multi-person)
-  float* oh = A.take<float>(3 * C); float* dh = A.take<float>(3 * C); float* nh = A.take<float>(C); float* fh = A.take<float>(C);
-  float* pts = A.take<float>(3 * C * S); float* cpts = A.take<float>(3 * C * S); float* cdirs = A.take<float>(3 * C * S);
-  float* z_h = A.take<float>(C * S); float* raw_h = A.take<float>(4 * C * S);
-  float* z_c = A.take<float>(C * S); float* raw_c = A.take<float>(4 * C * S); float* w_c = A.take<float>(C * S);
-  float* z_f = A.take<float>(C * Sb); float* raw_f = A.take<float>(4 * C * Sb);
-  float* z_bh = A.take<float>(C * Sb); float* raw_bh = A.take<float>(4 * C * Sb);   // bkg rows of the hit rays
-  float* z_m = A.take<float>(C * Sm); float* raw_m = A.take<float>(4 * C * Sm);
-  float* rgb_h = A.take<float>(3 * C); float* dep_h = A.take<float>(C); float* acc_h = A.take<float>(C);
-  float* rgb_s = A.take<float>(3 * C); float* dep_s = A.take<float>(C); float* acc_s = A.take<float>(C);
-  float* z_a[NM_MAX_ACTORS]; float* raw_a[NM_MAX_ACTORS];
-  float* zu_a[NM_MAX_ACTORS]; float* rawu_a[NM_MAX_ACTORS];      // the same rows, compacted to the rays any actor hits
-  float *flag = nullptr, *zeros = nullptr;
-  if (multi_person) {
-    for (int a = 0; a < n_actors; ++a) {
-      z_a[a] = A.take<float>(C * S); raw_a[a] = A.take<float>(4 * C * S);
-      zu_a[a] = A.take<float>(C * S); rawu_a[a] = A.take<float>(4 * C * S);
-    }
-    flag = A.take<float>(C); zeros = A.take<float>(C);
-  }
-
-  if (A.off > ctx->ws_bytes) NM_FAIL(ctx, NM_ERR_STATE, "render: workspace arena overflow (internal sizing bug)");
-  if (!ctx->ev_counts) NM_CHECK_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_counts, cudaEventDisableTiming));
-  for (int64_t i = 0; i < n; i += C) {
-    int64_t c = std::min<int64_t>(C, n - i);
-    TRY(nm_impl_raygen(ctx, cam, 0, pix0 + i, c, nullptr, pixels ? pixels + i : nullptr, o, d, st));                        // shot_rays (:271 / :386)
-    // Hit lists of every actor (:299 / :415) and, for several actors, of their union FIRST: the counts travel to the host
-    // while the background networks run, so the host never waits for them with the GPU idle.
-    int64_t Rh_a[NM_MAX_ACTORS]; int64_t Ru = 0;
-    NM_CHECK_CUDA(ctx, cudaMemsetAsync(ctx->d_counter, 0, sizeof(int32_t) * (n_actors + 1), st));
-    if (multi_person) { LAUNCH1D(k_fill, c, st, flag, c, 0.f); LAUNCH1D(k_fill, c, st, zeros, c, 0.f); }
-    for (int a = 0; a < n_actors; ++a) {
-      TRY(nm_impl_near_far_mesh(ctx, ctx->meshes[actors[a]], o, d, c, opt->geo_threshold, nr_a[a], fr_a[a], st));
-      LAUNCH1D(k_compact_hits, c, st, nr_a[a], fr_a[a], c, hit_a[a], ctx->d_counter + a);
-      if (multi_person) LAUNCH1D(k_mark_hits, c, st, nr_a[a], fr_a[a], c, flag);
-    }
-    if (multi_person) LAUNCH1D(k_compact_hits, c, st, zeros, flag, c, hit, ctx->d_counter + n_actors);
-    NM_CHECK_CUDA(ctx, cudaMemcpyAsync(ctx->h_counter, ctx->d_counter, sizeof(int32_t) * (n_actors + 1), cudaMemcpyDeviceToHost, st));
-    NM_CHECK_CUDA(ctx, cudaEventRecord(ctx->ev_counts, st));
-    float *raw_b, *z_b; int St;
-    TRY(bkg_pass(ctx, coarse_slot, fine_slot, opt, o, d, c, z_c, raw_c, w_c, z_f, raw_f, &raw_b, &z_b, &St, st));
-    NM_CHECK_CUDA(ctx, cudaEventSynchronize(ctx->ev_counts));
-    for (int a = 0; a < n_actors; ++a) { Rh_a[a] = ctx->h_counter[a]; ctx->last_hit_rays += Rh_a[a]; }
-    Ru = ctx->h_counter[n_actors];
-    float* rgb_dst = host_out ? rgb_s : rgb + 3 * i;
-    float* dep_dst = host_out ? dep_s : (depth ? depth + i : dep_s);
-    float* acc_dst = host_out ? acc_s : (acc ? acc + i : acc_s);
-    if (!multi_person) {
-      // all rays first get the background-only composite (miss rays keep it, :301-311)
-      TRY(nm_raw2outputs(ctx, raw_b, z_b, d, c, St, nullptr, 1.f, opt->white_bkg, rgb_dst, nullptr, nullptr, nullptr, dep_dst, st));
-      LAUNCH1D(k_fill, c, st, acc_dst, c, 0.f);
-      const int64_t Rh = Rh_a[0];
-      const int32_t* hit = hit_a[0];
-      const float *nr = nr_a[0], *fr = fr_a[0];
-      if (Rh > 0) {
-        LAUNCH1D(k_gather_rays, Rh, st, hit, (int)Rh, o, d, nr, fr, oh, dh, nh, fh);
-        TRY(human_branch(ctx, human_slots[0], actors[0], opt, oh, dh, nh, fh, Rh, pts, cpts, cdirs, z_h, raw_h, false, st));
-        LAUNCH1D(k_move_rows, Rh * St, st, hit, Rh, St, z_b, z_bh, 0);
-        LAUNCH1D(k_move_rows, Rh * St * 4, st, hit, Rh, St * 4, raw_b, raw_bh, 0);
-        const float* zl[2] = {z_bh, z_h};
-        const float* rl[2] = {raw_bh, raw_h};
-        const int32_t Sl[2] = {St, S};
-        TRY(nm_merge_samples(ctx, 2, zl, rl, Sl, Rh, z_m, raw_m, st));                  // (:330-337)
-        TRY(nm_raw2outputs(ctx, raw_m, z_m, dh, Rh, St + S, nullptr, 1.f, opt->white_bkg, rgb_h, nullptr, nullptr, nullptr,
-                           dep_h, st));                                                // (:338-343)
-        TRY(nm_raw2outputs(ctx, raw_h, z_h, dh, Rh, S, nullptr, 1.f, opt->white_bkg, nullptr, nullptr, acc_h, nullptr,
-                           nullptr, st));                                              // (:345-350)
-        LAUNCH1D(k_move_rows, Rh * 3, st, hit, Rh, 3, rgb_h, rgb_dst, 1);
-        LAUNCH1D(k_move_rows, Rh, st, hit, Rh, 1, dep_h, dep_dst, 1);
-        LAUNCH1D(k_move_rows, Rh, st, hit, Rh, 1, acc_h, acc_dst, 1);
+  const int Sb = S + N, Sm = Sb + n_actors * S;      // samples of the background and of the full merge
+  Hits h{n_actors, multi_person != 0, actors};
+  float *z_c, *raw_c, *w_c, *z_f, *raw_f, *z_bh, *raw_bh, *z_m, *raw_m;
+  float *z_a[NM_MAX_ACTORS], *raw_a[NM_MAX_ACTORS];
+  float *zu_a[NM_MAX_ACTORS], *rawu_a[NM_MAX_ACTORS];      // the same rows, compacted to the rays any actor hits
+  return render_frame(ctx, cam, opt, 0, pix0, n, pixels, Planes{rgb, depth, acc}, host_out, st,   // shot_rays (:271 / :386)
+    [&](Arena& A, int64_t C) {
+      h.take(A, C, S);
+      z_c = A.take<float>(C * S); raw_c = A.take<float>(4 * C * S); w_c = A.take<float>(C * S);
+      z_f = A.take<float>(C * Sb); raw_f = A.take<float>(4 * C * Sb);
+      z_bh = A.take<float>(C * Sb); raw_bh = A.take<float>(4 * C * Sb);   // bkg rows of the hit rays
+      z_m = A.take<float>(C * Sm); raw_m = A.take<float>(4 * C * Sm);
+      for (int a = 0; multi_person && a < n_actors; ++a) {
+        z_a[a] = A.take<float>(C * S); raw_a[a] = A.take<float>(4 * C * S);
+        zu_a[a] = A.take<float>(C * S); rawu_a[a] = A.take<float>(4 * C * S);
       }
-    } else {
+    },
+    [&](int64_t c, const float* o, const float* d, const Planes& dst) -> int {
+      // Hit lists FIRST: the counts travel to the host while the background networks run, so the host never waits
+      // for them with the GPU idle.
+      TRY(hit_lists(ctx, h, opt->geo_threshold, o, d, c, st));
+      float *raw_b, *z_b; int St;
+      TRY(bkg_pass(ctx, coarse_slot, fine_slot, opt, o, d, c, z_c, raw_c, w_c, z_f, raw_f, &raw_b, &z_b, &St, st));
+      TRY(hit_counts(ctx, h));
+      if (!multi_person) {
+        // all rays first get the background-only composite (miss rays keep it, :301-311)
+        TRY(nm_raw2outputs(ctx, raw_b, z_b, d, c, St, nullptr, 1.f, opt->white_bkg, dst.rgb, nullptr, nullptr, nullptr, dst.depth, st));
+        LAUNCH1D(k_fill, c, st, dst.acc, c, 0.f);
+        const int64_t Rh = h.count[0];
+        const int32_t* hit = h.idx[0];
+        if (Rh > 0) {
+          TRY(human_branch(ctx, human_slots[0], opt, o, d, h, 0, false, st));
+          LAUNCH1D(k_move_rows, Rh * St, st, hit, Rh, St, z_b, z_bh, 0);
+          LAUNCH1D(k_move_rows, Rh * St * 4, st, hit, Rh, St * 4, raw_b, raw_bh, 0);
+          const float* zl[2] = {z_bh, h.z};
+          const float* rl[2] = {raw_bh, h.raw};
+          const int32_t Sl[2] = {St, S};
+          TRY(nm_merge_samples(ctx, 2, zl, rl, Sl, Rh, z_m, raw_m, st));                  // (:330-337)
+          TRY(nm_raw2outputs(ctx, raw_m, z_m, h.dh, Rh, St + S, nullptr, 1.f, opt->white_bkg, h.rgb, nullptr, nullptr, nullptr,
+                             h.depth, st));                                                // (:338-343)
+          TRY(nm_raw2outputs(ctx, h.raw, h.z, h.dh, Rh, S, nullptr, 1.f, opt->white_bkg, nullptr, nullptr, h.acc, nullptr,
+                             nullptr, st));                                              // (:345-350)
+          LAUNCH1D(k_move_rows, Rh * 3, st, hit, Rh, 3, h.rgb, dst.rgb, 1);
+          LAUNCH1D(k_move_rows, Rh, st, hit, Rh, 1, h.depth, dst.depth, 1);
+          LAUNCH1D(k_move_rows, Rh, st, hit, Rh, 1, h.acc, dst.acc, 1);
+        }
+        return NM_OK;
+      }
       // Rays no actor hits carry only zero-density placeholders behind the background samples (:418-419): their
       // composite is the background composite whose last interval ends at the first placeholder (z = 2 far), no
       // sort needed.  Rays at least one actor hits go through the full z-sorted merge (:441-448), compacted.
-      TRY(nm_impl_raw2outputs_zend(ctx, raw_b, z_b, d, c, St, opt->white_bkg, opt->far_bkg * 2.f, rgb_dst, dep_dst, st));
+      TRY(nm_impl_raw2outputs_zend(ctx, raw_b, z_b, d, c, St, opt->white_bkg, opt->far_bkg * 2.f, dst.rgb, dst.depth, st));
       for (int a = 0; a < n_actors; ++a) {
         LAUNCH1D(k_fill_placeholder, c * S, st, z_a[a], (float4*)raw_a[a], c, S, opt->far_bkg * 2.f, opt->far_bkg * 3.f);
-        const int64_t Rh = Rh_a[a];
+        const int64_t Rh = h.count[a];
         if (Rh > 0) {
-          LAUNCH1D(k_gather_rays, Rh, st, hit_a[a], (int)Rh, o, d, nr_a[a], fr_a[a], oh, dh, nh, fh);
-          TRY(human_branch(ctx, human_slots[a], actors[a], opt, oh, dh, nh, fh, Rh, pts, cpts, cdirs, z_h, raw_h, false, st));
-          LAUNCH1D(k_move_rows, Rh * S, st, hit_a[a], Rh, S, z_h, z_a[a], 1);              // (:438-439)
-          LAUNCH1D(k_move_rows, Rh * S * 4, st, hit_a[a], Rh, S * 4, raw_h, raw_a[a], 1);
+          TRY(human_branch(ctx, human_slots[a], opt, o, d, h, a, false, st));
+          LAUNCH1D(k_move_rows, Rh * S, st, h.idx[a], Rh, S, h.z, z_a[a], 1);              // (:438-439)
+          LAUNCH1D(k_move_rows, Rh * S * 4, st, h.idx[a], Rh, S * 4, h.raw, raw_a[a], 1);
         }
       }
+      const int64_t Ru = h.count[n_actors];
       if (Ru > 0) {
         const float* zl[1 + NM_MAX_ACTORS]; const float* rl[1 + NM_MAX_ACTORS]; int32_t Sl[1 + NM_MAX_ACTORS];
-        LAUNCH1D(k_gather_rays, Ru, st, hit, (int)Ru, o, d, zeros, flag, oh, dh, nh, fh);
-        LAUNCH1D(k_move_rows, Ru * St, st, hit, Ru, St, z_b, z_bh, 0);
-        LAUNCH1D(k_move_rows, Ru * St * 4, st, hit, Ru, St * 4, raw_b, raw_bh, 0);
+        LAUNCH1D(k_gather_rays, Ru, st, h.uidx, (int)Ru, o, d, h.zeros, h.flag, h.oh, h.dh, h.nh, h.fh);
+        LAUNCH1D(k_move_rows, Ru * St, st, h.uidx, Ru, St, z_b, z_bh, 0);
+        LAUNCH1D(k_move_rows, Ru * St * 4, st, h.uidx, Ru, St * 4, raw_b, raw_bh, 0);
         zl[0] = z_bh; rl[0] = raw_bh; Sl[0] = St;
         for (int a = 0; a < n_actors; ++a) {
-          LAUNCH1D(k_move_rows, Ru * S, st, hit, Ru, S, z_a[a], zu_a[a], 0);
-          LAUNCH1D(k_move_rows, Ru * S * 4, st, hit, Ru, S * 4, raw_a[a], rawu_a[a], 0);
+          LAUNCH1D(k_move_rows, Ru * S, st, h.uidx, Ru, S, z_a[a], zu_a[a], 0);
+          LAUNCH1D(k_move_rows, Ru * S * 4, st, h.uidx, Ru, S * 4, raw_a[a], rawu_a[a], 0);
           zl[1 + a] = zu_a[a]; rl[1 + a] = rawu_a[a]; Sl[1 + a] = S;
         }
-        TRY(nm_merge_samples(ctx, n_lists, zl, rl, Sl, Ru, z_m, raw_m, st));              // (:441-448)
-        TRY(nm_raw2outputs(ctx, raw_m, z_m, dh, Ru, Sm, nullptr, 1.f, opt->white_bkg, rgb_h, nullptr, nullptr, nullptr,
-                           dep_h, st));                                                // (:449-454)
-        LAUNCH1D(k_move_rows, Ru * 3, st, hit, Ru, 3, rgb_h, rgb_dst, 1);
-        LAUNCH1D(k_move_rows, Ru, st, hit, Ru, 1, dep_h, dep_dst, 1);
+        TRY(nm_merge_samples(ctx, 1 + n_actors, zl, rl, Sl, Ru, z_m, raw_m, st));         // (:441-448)
+        TRY(nm_raw2outputs(ctx, raw_m, z_m, h.dh, Ru, Sm, nullptr, 1.f, opt->white_bkg, h.rgb, nullptr, nullptr, nullptr,
+                           h.depth, st));                                                // (:449-454)
+        LAUNCH1D(k_move_rows, Ru * 3, st, h.uidx, Ru, 3, h.rgb, dst.rgb, 1);
+        LAUNCH1D(k_move_rows, Ru, st, h.uidx, Ru, 1, h.depth, dst.depth, 1);
       }
-      LAUNCH1D(k_fill, c, st, acc_dst, c, 0.f);
-    }
-    if (host_out) {
-      TRY(copy_out(ctx, rgb + 3 * i, rgb_s, 3 * c, 1, st));
-      if (depth) TRY(copy_out(ctx, depth + i, dep_s, c, 1, st));
-      if (acc) TRY(copy_out(ctx, acc + i, acc_s, c, 1, st));
-      NM_CHECK_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-  }
-  return NM_OK;
+      LAUNCH1D(k_fill, c, st, dst.acc, c, 0.f);
+      return NM_OK;
+    });
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -20,10 +20,15 @@ def _mlp_mode():
     return _lib.NM_MLP_SIMT_F32 if os.environ.get("NEUMAN_MLP_MODE", "tc") == "simt" else _lib.NM_MLP_TC_F16
 
 
+def _device_ctx(device):
+    """The library context of a CUDA torch.device; a device without an index is the current one."""
+    return Context.get(device.index if device.index is not None else torch.cuda.current_device())
+
+
 def _ctx_for(t):
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
         raise RuntimeError("neuman_b200 ops need CUDA tensors (no CPU fallback)")
-    return Context.get(t.device.index if t.device.index is not None else torch.cuda.current_device())
+    return _device_ctx(t.device)
 
 
 def _f32(t, device=None):
@@ -183,10 +188,10 @@ def camera_struct(cap):
 def shot_rays(cap, xys, device=None):
     """utils/ray_utils.py:23-29 -> (origins, dirs) float32 CUDA tensors [n,3]."""
     device = torch.device(device or "cuda")
-    ctx = Context.get(device.index if device.index is not None else torch.cuda.current_device())
+    ctx = _device_ctx(device)
     if isinstance(xys, torch.Tensor) and xys.is_cuda:           # already on the device (neuman_b200/data.py)
         device = xys.device
-        ctx = Context.get(device.index if device.index is not None else torch.cuda.current_device())
+        ctx = _device_ctx(device)
         xy = xys[:, :2].to(torch.int32).contiguous()
     else:
         xy = torch.as_tensor(np.ascontiguousarray(np.asarray(xys)[:, :2]).astype(np.int32)).to(device)
@@ -202,7 +207,7 @@ def shot_rays(cap, xys, device=None):
 def shot_all_rays(cap, device=None, mode=1):
     """utils/ray_utils.py:32-38 (+ the .float() of render_utils.py:114-115)."""
     device = torch.device(device or "cuda")
-    ctx = Context.get(device.index if device.index is not None else torch.cuda.current_device())
+    ctx = _device_ctx(device)
     n = int(cap.shape[0]) * int(cap.shape[1])
     o = torch.empty(n, 3, device=device)
     d = torch.empty(n, 3, device=device)
@@ -347,7 +352,7 @@ def set_mesh(verts, faces, T, actor=0, device=None):
     CUDA tensors are taken from device memory, anything else goes through host arrays."""
     if isinstance(verts, torch.Tensor) and verts.is_cuda:
         device = verts.device
-        ctx = Context.get(device.index if device.index is not None else torch.cuda.current_device())
+        ctx = _device_ctx(device)
         v = verts.detach().float().contiguous()
         f = faces_device(faces, device)
         t = None
@@ -359,7 +364,7 @@ def set_mesh(verts, faces, T, actor=0, device=None):
                                           0 if t is None else t.shape[0], 1, ctx.stream()))
         return ctx
     device = torch.device(device or "cuda")
-    ctx = Context.get(device.index if device.index is not None else torch.cuda.current_device())
+    ctx = _device_ctx(device)
     v = np.ascontiguousarray(verts.detach().cpu().numpy() if isinstance(verts, torch.Tensor) else verts, dtype=np.float32)
     f = np.ascontiguousarray(np.asarray(faces)[:, :3], dtype=np.int32)
     tp, tn = None, 0
@@ -468,7 +473,7 @@ class SmplModelDevice:
 
 def smpl_verts_transformations(model, poses, betas, concat_joints=False):
     """SMPL.verts_transformations (models/smpl.py:109-162) -> (vertices [V(+J),3], T [V(+J),4,4]) float32 CUDA."""
-    ctx = Context.get(model.device.index if model.device.index is not None else torch.cuda.current_device())
+    ctx = _device_ctx(model.device)
     pose = _f32(poses, model.device).reshape(-1)
     beta = _f32(betas, model.device).reshape(-1)
     n = model.n_verts + (model.n_joints if concat_joints else 0)
@@ -483,7 +488,7 @@ def smpl_verts_transformations(model, poses, betas, concat_joints=False):
 def smpl_scene_transforms(model, pose, betas, alignment, scale):
     """data_io/neuman_helper.py:299-330: returns (world_verts [V,3] f32, world_joints [J,3] f32,
     T_da2scene [V+J,4,4] f64) on the device."""
-    ctx = Context.get(model.device.index if model.device.index is not None else torch.cuda.current_device())
+    ctx = _device_ctx(model.device)
     p = _f32(pose, model.device).reshape(-1)
     da = torch.zeros(model.n_joints, 3, device=model.device)
     da[1, 2], da[2, 2] = 1.0, -1.0                                  # the 'da' pose (:293-297)

@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
-from ._lib import Context, NmRenderOpts
+from ._lib import NmRenderOpts
 
 DEFAULT_GEO_THRESH = ops.DEFAULT_GEO_THRESH
 CHUNK = 32768            # device-side rays per chunk
@@ -30,12 +30,6 @@ def _opts(S, N, white_bkg, near=0.0, far=1.0, geo=DEFAULT_GEO_THRESH, render_can
     o.near_bkg, o.far_bkg = float(near), float(far)
     o.geo_threshold, o.interval_comp = float(geo), float(interval_comp)
     return o
-
-
-def _ctx(device):
-    if device.type != "cuda":
-        raise RuntimeError("neuman_b200 renderers need the networks on a CUDA device (no CPU fallback)")
-    return Context.get(device.index if device.index is not None else torch.cuda.current_device())
 
 
 def _range_policy(ctx):
@@ -85,26 +79,36 @@ def _outputs(out, n, host_out, device, with_acc):
     return (torch.empty(n, 3, device=device), torch.empty(n, device=device)) + ((torch.empty(n, device=device),) if with_acc else ())
 
 
+def _render(device, cap, pix0, n, pixels, out, host_out, planes, driver):
+    """The part every range renderer shares: resolves the pixel range or list, provides the output tensors (planes = 2:
+    rgb, depth; 3: + acc), runs driver(ctx, cam, n, pixels, *outputs) under the device guard and applies the range
+    policy after a host-output call.  `driver` holds the driver-specific part (net slots, meshes, options, the ctypes
+    call with the pointers it is given) and returns the call's status.  Returns the output tensors."""
+    if device.type != "cuda":
+        raise RuntimeError("neuman_b200 renderers need the networks on a CUDA device (no CPU fallback)")
+    ctx = ops._device_ctx(device)
+    n, pix = _pixel_args(pixels, cap, pix0, n, device)
+    with torch.cuda.device(device):
+        outs = _outputs(out, n, host_out, device, planes == 3)[:planes]
+        ctx.check(driver(ctx, ops.camera_struct(cap), n, ops._p(pix), *map(ops._p, outs)))
+        if host_out:
+            _range_policy(ctx)
+    return outs
+
+
 def render_vanilla_range(coarse_net, cap, fine_net=None, samples_per_ray=64, importance_samples_per_ray=128,
                          white_bkg=True, near_far_source='bkg', pix0=0, n=None, host_out=True, chunk=CHUNK, pixels=None,
                          out=None):
     """Renders the row-major pixel range [pix0, pix0+n), or the pixel list `pixels` (int32 CUDA tensor). host_out: pinned
     host tensors (device->host copy inside the call) else CUDA tensors. Returns (rgb [n,3], depth [n])."""
-    device = _device_of(coarse_net)
-    ctx = _ctx(device)
-    n, pix = _pixel_args(pixels, cap, pix0, n, device)
-    with torch.cuda.device(device):
+    def driver(ctx, cam, n, pix, rgb, depth):
         cs = ops.net_slot(coarse_net, ctx)
         fs = ops.net_slot(fine_net, ctx) if fine_net is not None else -1
-        cam = ops.camera_struct(cap)
         o = _opts(samples_per_ray, importance_samples_per_ray if fine_net is not None else 0, white_bkg,
                   cap.near[near_far_source], cap.far[near_far_source], chunk=chunk)
-        rgb, depth = _outputs(out, n, host_out, device, False)[:2]
-        ctx.check(ctx.lib.nm_render_vanilla(ctx.h, cs, fs, C.byref(cam), C.byref(o), pix0, n, ops._p(pix), ops._p(rgb),
-                                            ops._p(depth), int(host_out), ctx.stream()))
-        if host_out:
-            _range_policy(ctx)
-    return rgb, depth
+        return ctx.lib.nm_render_vanilla(ctx.h, cs, fs, C.byref(cam), C.byref(o), pix0, n, pix, rgb, depth, int(host_out),
+                                         ctx.stream())
+    return _render(_device_of(coarse_net), cap, pix0, n, pixels, out, host_out, 2, driver)
 
 
 def render_vanilla(coarse_net, cap, fine_net=None, rays_per_batch=32768, samples_per_ray=64,
@@ -126,22 +130,17 @@ def render_smpl_nerf_range(net, cap, posed_verts, faces, Ts, samples_per_ray=64,
                            geo_threshold=DEFAULT_GEO_THRESH, interval_comp=1.0, pix0=0, n=None, host_out=True,
                            chunk=SMPL_CHUNK, pixels=None, out=None):
     device = _device_of(net)
-    ctx = _ctx(device)
-    n, pix = _pixel_args(pixels, cap, pix0, n, device)
-    with torch.cuda.device(device):
+    if Ts is None:      # canonical rendering never reads T (utils/render_utils.py:214-216)
+        Ts = np.tile(np.eye(4)[None], (np.asarray(posed_verts).shape[0], 1, 1))
+
+    def driver(ctx, cam, n, pix, rgb, depth, acc):
         hs = ops.net_slot(net.coarse_human_net, ctx)
-        if Ts is None:      # canonical rendering never reads T (utils/render_utils.py:214-216)
-            Ts = np.tile(np.eye(4)[None], (np.asarray(posed_verts).shape[0], 1, 1))
         ops.set_mesh(posed_verts, faces, Ts, 0, device)
-        cam = ops.camera_struct(cap)
         o = _opts(samples_per_ray, 0, white_bkg, geo=geo_threshold, render_can=render_can, interval_comp=interval_comp,
                   chunk=chunk)
-        rgb, depth, acc = _outputs(out, n, host_out, device, True)
-        ctx.check(ctx.lib.nm_render_smpl_nerf(ctx.h, hs, 0, C.byref(cam), C.byref(o), pix0, n, ops._p(pix), ops._p(rgb),
-                                              ops._p(depth), ops._p(acc), int(host_out), ctx.stream()))
-        if host_out:
-            _range_policy(ctx)
-    return rgb, depth, acc
+        return ctx.lib.nm_render_smpl_nerf(ctx.h, hs, 0, C.byref(cam), C.byref(o), pix0, n, pix, rgb, depth, acc,
+                                           int(host_out), ctx.stream())
+    return _render(device, cap, pix0, n, pixels, out, host_out, 3, driver)
 
 
 def render_smpl_nerf(net, cap, posed_verts, faces, Ts, rays_per_batch=32768, samples_per_ray=64, white_bkg=True,
@@ -164,9 +163,8 @@ def render_smpl_nerf(net, cap, posed_verts, faces, Ts, rays_per_batch=32768, sam
 def _hybrid(bkg_model, human_models, cap, posed_verts, faces, Ts, S, N, white_bkg, geo, multi, pix0, n, host_out, chunk,
             pixels=None, out=None):
     device = _device_of(bkg_model)
-    ctx = _ctx(device)
-    n, pix = _pixel_args(pixels, cap, pix0, n, device)
-    with torch.cuda.device(device):
+
+    def driver(ctx, cam, n, pix, rgb, depth, acc):
         cs = ops.net_slot(bkg_model.coarse_bkg_net, ctx)
         fs = ops.net_slot(bkg_model.fine_bkg_net, ctx) if bkg_model.fine_bkg_net is not None else -1
         na = len(human_models)
@@ -174,14 +172,10 @@ def _hybrid(bkg_model, human_models, cap, posed_verts, faces, Ts, S, N, white_bk
         ac = (C.c_int32 * na)(*range(na))
         for a in range(na):
             ops.set_mesh(posed_verts[a], faces[a], Ts[a], a, device)
-        cam = ops.camera_struct(cap)
         o = _opts(S, N if fs >= 0 else 0, white_bkg, cap.near['bkg'], cap.far['bkg'], geo=geo, chunk=chunk)
-        rgb, depth, acc = _outputs(out, n, host_out, device, True)
-        ctx.check(ctx.lib.nm_render_hybrid(ctx.h, cs, fs, na, hs, ac, int(multi), C.byref(cam), C.byref(o), pix0, n,
-                                           ops._p(pix), ops._p(rgb), ops._p(depth), ops._p(acc), int(host_out), ctx.stream()))
-        if host_out:
-            _range_policy(ctx)
-    return rgb, depth, acc
+        return ctx.lib.nm_render_hybrid(ctx.h, cs, fs, na, hs, ac, int(multi), C.byref(cam), C.byref(o), pix0, n, pix, rgb,
+                                        depth, acc, int(host_out), ctx.stream())
+    return _render(device, cap, pix0, n, pixels, out, host_out, 3, driver)
 
 
 def render_hybrid_nerf_range(net, cap, posed_verts, faces, Ts, samples_per_ray=64, importance_samples_per_ray=128,

@@ -78,8 +78,7 @@ class TilePartition:
         """One all_gather of the equal-sized shards + the un-permute kernel.  Returns the row-major frame planes
         (rgb [HW,3], depth [HW], acc [HW] | None) on every rank; the tensors are reused by the next call."""
         from . import ops
-        from ._lib import Context
-        ctx = Context.get(self.device.index if self.device.index is not None else torch.cuda.current_device())
+        ctx = ops._device_ctx(self.device)
         planes = self._planes
         if self.world > 1:
             import torch.distributed as dist

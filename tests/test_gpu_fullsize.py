@@ -190,11 +190,16 @@ def test_pixel_lists_match_ranges(nets, human):
     H, W = 72, 100                                                  # edge tiles are clipped (100 = 6*16 + 4, 72 = 4*16 + 8)
     K, c2w = scenes.camera(H, W, focal=90.0, seed=0)
     cap = nb.SimpleCapture(K, c2w, H, W, 0.0, 3.14)
-    b1, _ = util.bodies()
+    b1, b2 = util.bodies()
     geo = b1["geo_threshold"]
+
+    def multi(**kw):                                                # the multi-person driver, device output
+        return render._hybrid(human, [human, human], cap, [b1["verts"], b2["verts"]], [b1["faces"]] * 2, [b1["Ts"], b2["Ts"]],
+                              32, 32, True, geo, True, 0, None, False, render.CHUNK, **kw)
     full_v = render.render_vanilla_range(nets[0], cap, nets[1], 32, 32, host_out=False)
     full_h = render.render_hybrid_nerf_range(human, cap, b1["verts"], b1["faces"], b1["Ts"], 32, 32, True, geo, host_out=False)
     full_s = render.render_smpl_nerf_range(human, cap, b1["verts"], b1["faces"], b1["Ts"], 32, True, False, geo, 1.0, host_out=False)
+    full_m = multi()
     seen = torch.zeros(H * W, dtype=torch.int32, device=DEV)
     for world in (1, 3):
         seen.zero_()
@@ -206,6 +211,9 @@ def test_pixel_lists_match_ranges(nets, human):
             render.render_vanilla_range(nets[0], cap, nets[1], 32, 32, pixels=part.pixels, host_out=False, out=(rgb, dep))
             assert torch.equal(rgb, full_v[0][idx]) and torch.equal(dep, full_v[1][idx])
             bufs = part.buffers()
+            multi(pixels=part.pixels, out=bufs)
+            for a, f in zip(bufs, full_m):
+                assert torch.equal(a, f[idx])
             render.render_hybrid_nerf_range(human, cap, b1["verts"], b1["faces"], b1["Ts"], 32, 32, True, geo, pixels=part.pixels,
                                             host_out=False, out=bufs)
             for a, f in zip(bufs, full_h):

@@ -158,6 +158,15 @@ def test_human_shard_chunk_invariance_and_determinism(human):
                                                  [b1["Ts"], b2["Ts"]], samples_per_ray=32, importance_samples_per_ray=32,
                                                  geo_threshold=geo, pix0=p0, n=n)
     assert np.array_equal(m_full.reshape(-1, 3)[p0:p0 + n], m_part)
+    # chunk invariance of the human-only and the multi-person drivers
+    s_full = render.render_smpl_nerf_range(human, cap, b1["verts"], b1["faces"], b1["Ts"], 32, True, False, geo, 1.0, host_out=False)
+    s_small = render.render_smpl_nerf_range(human, cap, b1["verts"], b1["faces"], b1["Ts"], 32, True, False, geo, 1.0, host_out=False,
+                                            chunk=777)
+    m_dev, m_small = (render._hybrid(human, [human, human], cap, [b1["verts"], b2["verts"]], [b1["faces"]] * 2, [b1["Ts"], b2["Ts"]],
+                                     32, 32, True, geo, True, 0, None, False, chunk) for chunk in (render.CHUNK, 777))
+    for a, b in zip(s_full + m_dev, s_small + m_small):
+        assert torch.equal(a, b)
+    assert np.array_equal(m_full.reshape(-1, 3), m_dev[0].cpu().numpy())
 
 
 def test_human_all_miss_frame(human):

@@ -1,12 +1,15 @@
-"""Bit-for-bit comparison of the tensor-core MLP forward between two builds of the library.
+"""Bit-for-bit comparison of the tensor-core MLP forward and the frame drivers between two builds of the library.
 
     python tools/fwd_digest.py dump OUT.json [--root TREE]     # run TREE's library (default: this tree) on seeded inputs
-    python tools/fwd_digest.py compare A.json B.json           # exit 1 unless every output is bit-identical
+    python tools/fwd_digest.py compare A.json B.json           # exit 1 unless every record is identical
 
 `dump` runs k_mlp_tc on seeded inputs and records a SHA-256 of every output buffer: the training forward's raw, activation
 stash (st_x, st_f, st_v) and sign words, and the inference raw in per-sample, per-ray-view and fused ray modes.  Sizes
-cover ragged tiles, several waves of the persistent grid and a frame-sized ray chunk.  Run it once from each build's
-tree (each loads its own libneuman_b200.so) and compare the two files."""
+cover ragged tiles, several waves of the persistent grid and a frame-sized ray chunk.  Its frames section renders with
+every driver (vanilla coarse-only and coarse + fine, smpl_nerf canonical and posed, hybrid, multi-person with 2 and 3
+actors), each with host and device output, a pixel range and a pixel list, the default chunk and a ragged one, and
+records the SHA-256 of rgb, depth and acc with the call's library launch count and render statistics.  Run it once from
+each build's tree (each loads its own libneuman_b200.so) and compare the two files."""
 import argparse
 import hashlib
 import json
@@ -70,10 +73,62 @@ def dump(out, root):
             raw = ops.mlp_forward_rays(j, o, d, z, mode=_lib.NM_MLP_TC_F16)
             torch.cuda.synchronize()
             res[f"{name}/rays/R={R}/S={S}/raw"] = _digest(raw)
+    frames(res, dev)
     _lib.Context.get(0).range_check()
     with open(out, "w") as f:
         json.dump(res, f, indent=1, sort_keys=True)
     print(f"{len(res) - 1} digests of {res['lib']} -> {out}")
+
+
+def frames(res, dev):
+    import torch
+    import neuman_b200 as nb
+    from neuman_b200 import _lib, render, sharding
+    from oracle import scenes, synth_smpl
+    ctx = _lib.Context.get(0)
+    coarse, fine = (m.to(dev) for m in scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False), 1))
+    torch.manual_seed(1)
+    human = nb.HumanNeRF(nb.default_opt(use_cuda=False))
+    scenes.boost_density(human.coarse_human_net)
+    human = human.to(dev)
+    H, W = 180, 240                                  # 43200 rays: two default chunks of the vanilla and hybrid drivers
+    K, c2w = scenes.camera(H, W, focal=200.0, seed=0)
+    cap = nb.SimpleCapture(K, c2w, H, W, 0.0, 3.14)
+    bodies = [synth_smpl.random_body(seed=s, center=c) for s, c in ((1, (0.1, 0.0, 0.3)), (4, (-0.15, 0.0, 0.5)),
+                                                                     (7, (0.35, 0.05, 0.7)))]
+    b, geo = bodies[0], bodies[0]["geo_threshold"]
+
+    def multi(k):
+        v, f, t = ([x[key] for x in bodies[:k]] for key in ("verts", "faces", "Ts"))
+
+        def run(pix0, n, host_out, chunk, pixels):
+            return render._hybrid(human, [human] * k, cap, v, f, t, 32, 32, True, geo, True, pix0, n, host_out, chunk, pixels=pixels)
+        return run
+    drivers = {
+        "vanilla_coarse": (lambda **kw: render.render_vanilla_range(coarse, cap, None, 32, 0, **kw), render.CHUNK),
+        "vanilla_fine": (lambda **kw: render.render_vanilla_range(coarse, cap, fine, 32, 32, **kw), render.CHUNK),
+        "smpl_canonical": (lambda **kw: render.render_smpl_nerf_range(human, cap, b["verts"], b["faces"], b["Ts"], 32, True, True,
+                                                                      geo, 0.7, **kw), render.SMPL_CHUNK),
+        "smpl_posed": (lambda **kw: render.render_smpl_nerf_range(human, cap, b["verts"], b["faces"], b["Ts"], 32, True, False,
+                                                                  geo, 0.7, **kw), render.SMPL_CHUNK),
+        "hybrid": (lambda **kw: render.render_hybrid_nerf_range(human, cap, b["verts"], b["faces"], b["Ts"], 32, 32, True, geo,
+                                                                **kw), render.CHUNK),
+        "multi2": (multi(2), render.CHUNK),
+        "multi3": (multi(3), render.CHUNK),
+    }
+    pixel_list = torch.from_numpy(sharding.tile_pixels(H, W, 1, 3)).to(dev)
+    for name, (fn, default_chunk) in drivers.items():
+        for host_out in (True, False):
+            for where, pix0, n, pixels in (("range", 1234, H * W - 1801, None), ("list", 0, None, pixel_list)):
+                for chunk in (default_chunk, 777):
+                    key = f"frames/{name}/host_out={int(host_out)}/{where}/chunk={chunk}"
+                    l0 = ctx.launch_count()
+                    outs = fn(pix0=pix0, n=n, host_out=host_out, chunk=chunk, pixels=pixels)
+                    torch.cuda.synchronize()
+                    res[key + "/launches"] = ctx.launch_count() - l0
+                    res[key + "/stats"] = ctx.render_stats()
+                    for plane, t in zip(("rgb", "depth", "acc"), outs):
+                        res[f"{key}/{plane}"] = _digest(t)
 
 
 def compare(a, b):
@@ -82,7 +137,7 @@ def compare(a, b):
     bad = [k for k in keys if A.get(k) != B.get(k)]
     for k in bad:
         print("DIFFERENT", k)
-    print(f"{len(keys) - len(bad)} of {len(keys)} outputs bit-identical ({A['lib']} vs {B['lib']})")
+    print(f"{len(keys) - len(bad)} of {len(keys)} records identical ({A['lib']} vs {B['lib']})")
     return 1 if bad else 0
 
 
