@@ -77,6 +77,27 @@ typedef struct {
  * Replaces nothing in the reference; it is the cost of `net.cuda()` / checkpoint load. */
 int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* desc, void* stream);
 
+/* A view-independent NeRF (use_viewdirs=False: the background nets' --use_viewdirs False, the canonical human net's
+ * --specular_can False; models/vanilla.py:117-118,145-146): the same 8x256 trunk with one output_linear [4,256] on
+ * layer 7 and no view-direction input.  fp32 DEVICE pointers in the reference's nn.Linear layout. */
+typedef struct {
+  const float* pts_w[8];
+  const float* pts_b[8];
+  const float* output_w;  const float* output_b;    /* output_linear [4,256], [4] */
+  int32_t pos_pe_kind;                              /* NM_PE_* for the position input */
+  float pos_min_freq, pos_max_freq; int32_t pos_n_freqs;
+} nm_nerf_noview_desc;
+
+/* Packs a view-independent net into `slot` (a slot may hold either kind; packing changes its kind).  Every entry point
+ * that takes a slot serves both kinds; for a view-independent slot:
+ *   nm_mlp_forward / nm_mlp_forward_rays: `views` may be NULL and is ignored, raw = output_linear(h7) (r, g, b, sigma);
+ *   nm_mlp_forward_train: stash_f and stash_v are NULL, stash_m has 8 planes [8][n][8] (pts_linears 0..7);
+ *   nm_mlp_backward: g_f and g_v are NULL (and stash_v is not read); g_pre as for view-dependent nets;
+ *   nm_dw_gemm: with NULL g_f, g_v and stash_f only out[0..6] (pts_linears 1..7) are computed, out[7..8] are zero;
+ *   nm_encode_f16 / nm_pe_backward with which = 1 return NM_ERR_UNSUPPORTED (there is no direction encoding);
+ *   the frame drivers accept any mix of kinds over their coarse, fine and human slots. */
+int nm_net_pack_noview(nm_ctx* ctx, int slot, const nm_nerf_noview_desc* desc, void* stream);
+
 /* Joiner.forward(input_pts, input_views) (models/vanilla.py:162-166) = Embedder.forward (:82-92)
  * on both inputs + NeRF.forward (:120-152).  pts, views: [n,3]; raw: [n,4].
  * If views_per_ray != 0, `views` is [n/views_per_ray, 3] and row i serves samples

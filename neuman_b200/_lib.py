@@ -26,6 +26,13 @@ class NmNerfDesc(C.Structure):
                 ("dir_min_freq", C.c_float), ("dir_max_freq", C.c_float), ("dir_n_freqs", C.c_int32)]
 
 
+class NmNerfNoviewDesc(C.Structure):
+    _fields_ = [("pts_w", C.c_void_p * 8), ("pts_b", C.c_void_p * 8),
+                ("output_w", C.c_void_p), ("output_b", C.c_void_p),
+                ("pos_pe_kind", C.c_int32),
+                ("pos_min_freq", C.c_float), ("pos_max_freq", C.c_float), ("pos_n_freqs", C.c_int32)]
+
+
 class NmCamera(C.Structure):
     _fields_ = [("K", C.c_double * 9), ("c2w", C.c_double * 16), ("H", C.c_int32), ("W", C.c_int32)]
 
@@ -54,6 +61,7 @@ SIGNATURES = {
     "nm_version": (C.c_char_p, []),
     "nm_launch_count": (_I64, [_P]),
     "nm_net_pack": (C.c_int, [_P, C.c_int, C.POINTER(NmNerfDesc), _P]),
+    "nm_net_pack_noview": (C.c_int, [_P, C.c_int, C.POINTER(NmNerfNoviewDesc), _P]),
     "nm_mlp_forward": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _I64, _I32, _P, _P]),
     "nm_mlp_forward_train": (C.c_int, [_P, C.c_int, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
     "nm_encode_f16": (C.c_int, [_P, C.c_int, _I32, _P, _I64, _I64, _P, _P]),

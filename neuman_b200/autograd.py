@@ -84,9 +84,12 @@ class _JoinerMLP(torch.autograd.Function):
         n = pts.shape[0]
         dev = pts.device
         h = dict(device=dev, dtype=torch.float16)
-        sx, sf = torch.empty(8, n, 256, **h), torch.empty(n, 256, **h)
-        sv = torch.empty(n, 128, **h)
-        sm = torch.empty(9, n, 8, device=dev, dtype=torch.int32)     # planes 0..7: pts_linears, 8: views layer
+        viewless = ops.is_viewless(joiner)
+        sx = torch.empty(8, n, 256, **h)
+        sf = sv = None                                                 # view-independent nets: no feature / views layer
+        if not viewless:
+            sf, sv = torch.empty(n, 256, **h), torch.empty(n, 128, **h)
+        sm = torch.empty(8 if viewless else 9, n, 8, device=dev, dtype=torch.int32)   # planes 0..7: pts_linears, 8: views layer
         raw = torch.empty(n, 4, device=dev, dtype=torch.float32)
         if n:
             ctx.check(ctx.lib.nm_mlp_forward_train(ctx.h, slot, _p(pts), _p(views), n, 0, _p(raw), _p(sx), _p(sf), _p(sv),
@@ -119,15 +122,17 @@ class _JoinerMLP(torch.autograd.Function):
         g = g_raw.reshape(-1, 4).float().contiguous()
         need_w = any(fctx.needs_input_grad[3:])
         d_pts = d_views = None
+        viewless = ops.is_viewless(joiner)
         if g.shape[0] == 0:
             grads = {k: torch.zeros_like(v) for k, v in P.items()}
-            d_pts, d_views = torch.zeros_like(pts), torch.zeros_like(views)
+            d_pts = torch.zeros_like(pts)
+            d_views = torch.zeros_like(views) if views is not None and not viewless else None
         else:
             g_pre, g_f, g_v, inv = _chain_kernel(joiner, P, stash, g)
             grads = _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv) if need_w else {}
             if fctx.needs_input_grad[0]:
                 d_pts = _input_grad(joiner, P, pts, 0, ((g_pre[0], 'pts_linears.0.weight', 0), (g_pre[5], 'pts_linears.5.weight', 0)), inv)
-            if fctx.needs_input_grad[1]:
+            if fctx.needs_input_grad[1] and not viewless:       # the views never reach the output of a view-independent net
                 d_views = _input_grad(joiner, P, views, 1, ((g_v, 'views_linears.0.weight', 256),), inv)
         out = [grads[k].reshape(P[k].shape).to(P[k].dtype) if fctx.needs_input_grad[3 + i] else None
                for i, k in enumerate(names)]
@@ -154,13 +159,16 @@ def _input_grad(joiner, P, x, which, terms, inv):
 
 
 def _encodings(joiner, pts, views):
-    """The fp16 encodings as the forward kernel multiplied them ([n,64] / [n,32], with their constant-1 channel)."""
+    """The fp16 encodings as the forward kernel multiplied them ([n,64] / [n,32], with their constant-1 channel); a
+    view-independent net has no direction encoding (None)."""
     ctx = _ctx_for(pts)
     slot = ops.net_slot(joiner, ctx)
     n = pts.shape[0]
     spe = torch.empty(n, 64, device=pts.device, dtype=torch.float16)
-    sdpe = torch.empty(n, 32, device=pts.device, dtype=torch.float16)
     ctx.check(ctx.lib.nm_encode_f16(ctx.h, slot, 0, _p(pts), 0, n, _p(spe), ctx.stream()))
+    if ops.is_viewless(joiner):
+        return spe, None
+    sdpe = torch.empty(n, 32, device=pts.device, dtype=torch.float16)
     ctx.check(ctx.lib.nm_encode_f16(ctx.h, slot, 1, _p(views), 0, n, _p(sdpe), ctx.stream()))
     return spe, sdpe
 
@@ -174,23 +182,29 @@ def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
     sx, sf, sv, _ = stash
     spe, sdpe = _encodings(joiner, pts, views)
     ctx = _ctx_for(g)
-    n_pe, n_dpe = joiner.pos_pe.out_dim, joiner.dir_pe.out_dim          # 63, 27: the 1.0 channel sits right after
+    n_pe = joiner.pos_pe.out_dim                                          # 63: the 1.0 channel sits right after
     grads = {}
     g8 = torch.zeros(g.shape[0], 8, device=g.device, dtype=torch.float16)
     g8[:, :4] = g * (1.0 / inv)
     g8t = g8.t()
-    grads['rgb_linear.weight'] = _mm32(g8t, sv)[:3] * inv
-    grads['rgb_linear.bias'] = g[:, :3].sum(0)
-    grads['alpha_linear.weight'] = _mm32(g8t, sx[7])[3:4] * inv
-    grads['alpha_linear.bias'] = g[:, 3].sum().reshape(1)
-    gvt = g_v.t()
-    wd = _mm32(gvt, sdpe) * inv                                           # [128, 32]
+    if ops.is_viewless(joiner):
+        # output_linear (models/vanilla.py:146) reads layer 7's output: g^T @ X7 in cuBLAS, as alpha_linear below
+        grads['output_linear.weight'] = _mm32(g8t, sx[7])[:4] * inv
+        grads['output_linear.bias'] = g.sum(0)
+    else:
+        n_dpe = joiner.dir_pe.out_dim                                     # 27
+        grads['rgb_linear.weight'] = _mm32(g8t, sv)[:3] * inv
+        grads['rgb_linear.bias'] = g[:, :3].sum(0)
+        grads['alpha_linear.weight'] = _mm32(g8t, sx[7])[3:4] * inv
+        grads['alpha_linear.bias'] = g[:, 3].sum().reshape(1)
     w0 = _mm32(g_pre[0].t(), spe) * inv                                   # [256,64]: column 63 = bias gradient (1.0 channel)
     dw, db = _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, g.shape[0])
     dw, db = dw * inv, db * inv
-    grads['views_linears.0.weight'] = torch.cat([dw[8, :128], wd[:, :n_dpe]], 1)
-    grads['views_linears.0.bias'] = db[8, :128]
-    grads['feature_linear.weight'], grads['feature_linear.bias'] = dw[7], db[7]
+    if sdpe is not None:
+        wd = _mm32(g_v.t(), sdpe) * inv                                   # [128, 32]
+        grads['views_linears.0.weight'] = torch.cat([dw[8, :128], wd[:, :n_dpe]], 1)
+        grads['views_linears.0.bias'] = db[8, :128]
+        grads['feature_linear.weight'], grads['feature_linear.bias'] = dw[7], db[7]
     for l in range(8):
         if l == 0:
             w = w0[:, :n_pe]
@@ -210,7 +224,9 @@ def _chain_kernel(joiner, P, stash, g):
     n = g.shape[0]
     scale = _pow2_scale(g, 256.0)
     h = dict(device=g.device, dtype=torch.float16)
-    g_pre, g_f, g_v = torch.empty(8, n, 256, **h), torch.empty(n, 256, **h), torch.empty(n, 128, **h)
+    g_pre, g_f, g_v = torch.empty(8, n, 256, **h), None, None
+    if not ops.is_viewless(joiner):                 # view-independent nets: no feature / views layer gradients
+        g_f, g_v = torch.empty(n, 256, **h), torch.empty(n, 128, **h)
     ctx.check(ctx.lib.nm_mlp_backward(ctx.h, slot, _p(g), _p(scale), n, _p(sv), _p(sm), _p(g_pre), _p(g_f), _p(g_v),
                                       ctx.stream()))
     return g_pre, g_f, g_v, 1.0 / scale
@@ -219,20 +235,23 @@ def _chain_kernel(joiner, P, stash, g):
 def _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, n):
     """The nine 256-wide weight gradients and their bias gradients, still carrying the loss scale of the g planes: one
     k_dw_gemm launch (csrc/dw_gemm.cu), every gradient and stash plane read once.
-    -> dw [9,256,256], db [9,256] fp32 (plane 8: rows 0..127 used)."""
+    -> dw [9,256,256], db [9,256] fp32 (plane 8: rows 0..127 used).  With g_f = g_v = sf = None (a view-independent net)
+    only planes 0..6 are computed."""
     dw = torch.empty(9, 256, 256, device=g_pre.device, dtype=torch.float32)
     db = torch.empty(9, 256, device=g_pre.device, dtype=torch.float32)
     ctx.check(ctx.lib.nm_dw_gemm(ctx.h, _p(g_pre), _p(g_f), _p(g_v), _p(sx), _p(sf), n, _p(dw), _p(db), ctx.stream()))
     return dw, db
 
 
-def joiner_forward(joiner, input_pts, input_views):
+def joiner_forward(joiner, input_pts, input_views=None):
     """Joiner.forward (models/vanilla.py:162-166) with gradients to the network parameters and, when they require
-    grad, to input_pts / input_views."""
+    grad, to input_pts / input_views.  A view-independent net ignores input_views (may be None); its gradient is None."""
     shape = input_pts.shape[:-1]
     pts = input_pts.float().contiguous().reshape(-1, 3)          # autograd-tracked views of the inputs
-    views = input_views.to(pts.device).float().contiguous().reshape(-1, 3)
-    assert views.shape[0] == pts.shape[0], "input_views must match input_pts"
+    views = None
+    if not ops.is_viewless(joiner):
+        views = input_views.to(pts.device).float().contiguous().reshape(-1, 3)
+        assert views.shape[0] == pts.shape[0], "input_views must match input_pts"
     params = [p for _, p in joiner.nerf.named_parameters()]
     return _JoinerMLP.apply(pts, views, joiner, *params).reshape(*shape, 4)
 

@@ -180,17 +180,11 @@ static void pe_cycles_table(int kind, float fmin, float fmax, int nf, std::vecto
     }
 }
 
-extern "C" int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* stream) {
-  NM_ENTER(ctx);
-  if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !d) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: bad slot/desc");
-  if (d->pos_n_freqs != 10 || d->dir_n_freqs != 4)
-    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_net_pack: only pos_N_freqs=10 / dir_N_freqs=4 (63/27-d encodings) is built");
-  for (int l = 0; l < 8; ++l)
-    if (!d->pts_w[l] || !d->pts_b[l]) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: null pts_linears");
-  if (!d->feature_w || !d->feature_b || !d->alpha_w || !d->alpha_b || !d->views_w || !d->views_b || !d->rgb_w ||
-      !d->rgb_b)
-    NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: null head weights (use_viewdirs=True nets only)");
-  cudaStream_t st = (cudaStream_t)stream;
+// Packs a validated description of either kind into `slot`.  For a view-independent net (kind NM_NET_NOVIEW) `d` carries
+// the trunk and the position encoding, its head pointers are null and its direction-encoding fields a fixed placeholder;
+// out_w / out_b are output_linear's weight and bias.
+static int net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, int kind, const float* out_w, const float* out_b,
+                    cudaStream_t st) {
   NmNet& n = ctx->nets[slot];
   if (!n.f32) {
     // layout (floats)
@@ -207,10 +201,12 @@ extern "C" int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* s
     n.o_rgb_w = take((size_t)NM_VIEWS_HID * 3); n.o_rgb_b = take(3);
     n.o_pos_bv = take(128); n.o_dir_bv = take(128);
     n.o_pos_cyc = take(192); n.o_dir_cyc = take(192);
+    n.o_out_w = take((size_t)NM_WIDTH * 4); n.o_out_b = take(4);
     n.f32_floats = off;
     NM_CHECK_CUDA(ctx, cudaMalloc(&n.f32, off * sizeof(float)));
   }
   n.desc = *d;
+  n.kind = kind;
   n.bwd_packed = false;
   auto tr = [&](const float* src, size_t dst_off, int n_out, int n_in) {
     int total = n_out * n_in;
@@ -225,14 +221,19 @@ extern "C" int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* s
     tr(d->pts_w[l], n.o_pts_w[l], NM_WIDTH, K);
     NM_CHECK_CUDA(ctx, cp(d->pts_b[l], n.o_pts_b[l], NM_WIDTH));
   }
-  tr(d->feature_w, n.o_feat_w, NM_WIDTH, NM_WIDTH);
-  NM_CHECK_CUDA(ctx, cp(d->feature_b, n.o_feat_b, NM_WIDTH));
-  tr(d->alpha_w, n.o_alpha_w, 1, NM_WIDTH);
-  NM_CHECK_CUDA(ctx, cp(d->alpha_b, n.o_alpha_b, 1));
-  tr(d->views_w, n.o_views_w, NM_VIEWS_HID, NM_WIDTH + NM_DIR_PE);
-  NM_CHECK_CUDA(ctx, cp(d->views_b, n.o_views_b, NM_VIEWS_HID));
-  tr(d->rgb_w, n.o_rgb_w, 3, NM_VIEWS_HID);
-  NM_CHECK_CUDA(ctx, cp(d->rgb_b, n.o_rgb_b, 3));
+  if (kind == NM_NET_VIEW) {
+    tr(d->feature_w, n.o_feat_w, NM_WIDTH, NM_WIDTH);
+    NM_CHECK_CUDA(ctx, cp(d->feature_b, n.o_feat_b, NM_WIDTH));
+    tr(d->alpha_w, n.o_alpha_w, 1, NM_WIDTH);
+    NM_CHECK_CUDA(ctx, cp(d->alpha_b, n.o_alpha_b, 1));
+    tr(d->views_w, n.o_views_w, NM_VIEWS_HID, NM_WIDTH + NM_DIR_PE);
+    NM_CHECK_CUDA(ctx, cp(d->views_b, n.o_views_b, NM_VIEWS_HID));
+    tr(d->rgb_w, n.o_rgb_w, 3, NM_VIEWS_HID);
+    NM_CHECK_CUDA(ctx, cp(d->rgb_b, n.o_rgb_b, 3));
+  } else {
+    tr(out_w, n.o_out_w, 4, NM_WIDTH);
+    NM_CHECK_CUDA(ctx, cp(out_b, n.o_out_b, 4));
+  }
   NM_CHECK_CUDA(ctx, cudaGetLastError());
   // encoding tables: host-built, uploaded (with a sync, `tab` is a temporary) only when the description changes,
   // so that re-packing updated weights every training step stays asynchronous
@@ -265,6 +266,36 @@ extern "C" int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* s
   if (rc != NM_OK) return rc;
   n.packed = true;
   return NM_OK;
+}
+
+extern "C" int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* stream) {
+  NM_ENTER(ctx);
+  if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !d) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: bad slot/desc");
+  if (d->pos_n_freqs != 10 || d->dir_n_freqs != 4)
+    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_net_pack: only pos_N_freqs=10 / dir_N_freqs=4 (63/27-d encodings) is built");
+  for (int l = 0; l < 8; ++l)
+    if (!d->pts_w[l] || !d->pts_b[l]) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: null pts_linears");
+  if (!d->feature_w || !d->feature_b || !d->alpha_w || !d->alpha_b || !d->views_w || !d->views_b || !d->rgb_w ||
+      !d->rgb_b)
+    NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: null head weights (use_viewdirs=True nets only)");
+  return net_pack(ctx, slot, d, NM_NET_VIEW, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int nm_net_pack_noview(nm_ctx* ctx, int slot, const nm_nerf_noview_desc* d, void* stream) {
+  NM_ENTER(ctx);
+  if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !d) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack_noview: bad slot/desc");
+  if (d->pos_n_freqs != 10)
+    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_net_pack_noview: only pos_N_freqs=10 (63-d encoding) is built");
+  for (int l = 0; l < 8; ++l)
+    if (!d->pts_w[l] || !d->pts_b[l]) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack_noview: null pts_linears");
+  if (!d->output_w || !d->output_b) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack_noview: null output_linear");
+  nm_nerf_desc full{};
+  for (int l = 0; l < 8; ++l) { full.pts_w[l] = d->pts_w[l]; full.pts_b[l] = d->pts_b[l]; }
+  full.pos_pe_kind = d->pos_pe_kind;
+  full.pos_min_freq = d->pos_min_freq; full.pos_max_freq = d->pos_max_freq; full.pos_n_freqs = d->pos_n_freqs;
+  // no direction input: the placeholder only keeps the (unused) direction tables of the slot well defined
+  full.dir_pe_kind = NM_PE_POSENC; full.dir_min_freq = 0.f; full.dir_max_freq = 3.f; full.dir_n_freqs = 4;
+  return net_pack(ctx, slot, &full, NM_NET_NOVIEW, d->output_w, d->output_b, (cudaStream_t)stream);
 }
 
 static int mlp_dispatch(nm_ctx* ctx, int slot, int mode, const float* pts, const float* views, const float* origins,
@@ -300,10 +331,18 @@ static int mlp_dispatch(nm_ctx* ctx, int slot, int mode, const float* pts, const
   return rc;
 }
 
+// views of a view-independent slot are never read and may be NULL
+static bool views_ok(const nm_ctx* ctx, int slot, const void* views) {
+  return views || (slot >= 0 && slot < NM_MAX_NET_SLOTS && ctx->nets[slot].packed && ctx->nets[slot].kind == NM_NET_NOVIEW);
+}
+static bool is_noview(const nm_ctx* ctx, int slot) {
+  return slot >= 0 && slot < NM_MAX_NET_SLOTS && ctx->nets[slot].kind == NM_NET_NOVIEW;
+}
+
 extern "C" int nm_mlp_forward(nm_ctx* ctx, int slot, int mode, const float* pts, const float* views, int64_t n,
                               int32_t views_per_ray, float* raw, void* stream) {
   NM_ENTER(ctx);
-  if (!pts || !views || views_per_ray < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward: null pts/views");
+  if (!pts || !views_ok(ctx, slot, views) || views_per_ray < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward: null pts/views");
   if (views_per_ray > 0 && n % views_per_ray != 0)
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward: n is not a multiple of views_per_ray");
   return mlp_dispatch(ctx, slot, mode, pts, views, nullptr, nullptr, nullptr, n, views_per_ray, raw, stream);
@@ -313,9 +352,11 @@ extern "C" int nm_mlp_forward_train(nm_ctx* ctx, int slot, const float* pts, con
                                     int32_t views_per_ray, float* raw, void* stash_x, void* stash_f, void* stash_v,
                                     void* stash_m, void* stream) {
   NM_ENTER(ctx);
-  if (!pts || !views || views_per_ray < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_train: null pts/views");
-  if (!stash_x || !stash_f || !stash_v || !stash_m)
+  if (!pts || !views_ok(ctx, slot, views) || views_per_ray < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_train: null pts/views");
+  const bool noview = is_noview(ctx, slot);
+  if (!stash_x || !stash_m || (!noview && (!stash_f || !stash_v)))
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_train: null stash");
+  if (noview) stash_f = stash_v = nullptr;
   if (views_per_ray > 0 && n % views_per_ray != 0)
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_train: n is not a multiple of views_per_ray");
   NmTrainStash sh{(__half*)stash_x, (__half*)stash_f, (__half*)stash_v, (uint32_t*)stash_m};
@@ -329,8 +370,10 @@ extern "C" int nm_mlp_backward(nm_ctx* ctx, int slot, const float* d_raw, const 
     NM_FAIL(ctx, NM_ERR_STATE, "nm_mlp_backward: net slot not packed");
   if (n < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_backward: bad argument");
   if (n == 0) return NM_OK;
-  if (!d_raw || !loss_scale || !stash_v || !stash_m || !g_pre || !g_f || !g_v)
+  const bool noview = is_noview(ctx, slot);
+  if (!d_raw || !loss_scale || !stash_m || !g_pre || (!noview && (!stash_v || !g_f || !g_v)))
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_backward: null argument");
+  if (noview) stash_v = g_f = g_v = nullptr;
   return nm_tc_backward(ctx, ctx->nets[slot], d_raw, loss_scale, n, (const __half*)stash_v, (const uint32_t*)stash_m,
                         (__half*)g_pre, (__half*)g_f, (__half*)g_v, (cudaStream_t)stream);
 }
@@ -341,6 +384,7 @@ extern "C" int nm_encode_f16(nm_ctx* ctx, int slot, int32_t which, const float* 
   if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !ctx->nets[slot].packed)
     NM_FAIL(ctx, NM_ERR_STATE, "nm_encode_f16: net slot not packed");
   if ((which != 0 && which != 1) || n < 0 || group < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_encode_f16: bad argument");
+  if (which == 1 && is_noview(ctx, slot)) NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_encode_f16: view-independent net has no direction encoding");
   if (n == 0) return NM_OK;
   if (!x || !out) NM_FAIL(ctx, NM_ERR_INVALID, "nm_encode_f16: null argument");
   return nm_tc_encode(ctx, ctx->nets[slot], which, x, group, n, (__half*)out, (cudaStream_t)stream);
@@ -352,6 +396,7 @@ extern "C" int nm_pe_backward(nm_ctx* ctx, int slot, int32_t which, const float*
   if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !ctx->nets[slot].packed)
     NM_FAIL(ctx, NM_ERR_STATE, "nm_pe_backward: net slot not packed");
   if ((which != 0 && which != 1) || n < 0 || group < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_pe_backward: bad argument");
+  if (which == 1 && is_noview(ctx, slot)) NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_pe_backward: view-independent net has no direction encoding");
   const NmNet& net = ctx->nets[slot];
   const int width = 3 + 6 * (which == 0 ? net.desc.pos_n_freqs : net.desc.dir_n_freqs);
   if (ld < width) NM_FAIL(ctx, NM_ERR_INVALID, "nm_pe_backward: ld smaller than the encoding width");
@@ -369,7 +414,9 @@ extern "C" int nm_dw_gemm(nm_ctx* ctx, const void* g_pre, const void* g_f, const
     NM_CHECK_CUDA(ctx, cudaMemsetAsync(bias_out, 0, (size_t)9 * 256 * sizeof(float), (cudaStream_t)stream));
     return NM_OK;
   }
-  if (!g_pre || !g_f || !g_v || !stash_x || !stash_f) NM_FAIL(ctx, NM_ERR_INVALID, "nm_dw_gemm: null argument");
+  // g_f, g_v and stash_f all NULL: a view-independent net's backward (items 0..6 only)
+  const bool trunk_only = !g_f && !g_v && !stash_f;
+  if (!g_pre || !stash_x || (!trunk_only && (!g_f || !g_v || !stash_f))) NM_FAIL(ctx, NM_ERR_INVALID, "nm_dw_gemm: null argument");
   return nm_impl_dw_gemm(ctx, (const __half*)g_pre, (const __half*)g_f, (const __half*)g_v, (const __half*)stash_x,
                          (const __half*)stash_f, n, out, bias_out, (cudaStream_t)stream);
 }

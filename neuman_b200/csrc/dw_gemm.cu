@@ -146,9 +146,13 @@ int nm_impl_dw_gemm(nm_ctx* ctx, const __half* g_pre, const __half* g_f, const _
   DwParams P;
   memset(&P, 0, sizeof(P));
   const CUtensorMapL2promotion l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
-  if (tc_make_map(&P.maps[0], g_pre, 8, (uint64_t)n, 256, DW_ROWS, l2) || tc_make_map(&P.maps[1], g_f, 1, (uint64_t)n, 256, DW_ROWS, l2) ||
-      tc_make_map(&P.maps[2], g_v, 1, (uint64_t)n, 128, DW_ROWS, l2) || tc_make_map(&P.maps[3], st_x, 8, (uint64_t)n, 256, DW_ROWS, l2) ||
-      tc_make_map(&P.maps[4], st_f, 1, (uint64_t)n, 256, DW_ROWS, l2))
+  // a view-independent net (no feature / views layers: g_f, g_v, st_f null) has the seven trunk items 0..6 only
+  const bool trunk_only = !g_f;
+  const int n_items = trunk_only ? 7 : DW_ITEMS;
+  if (tc_make_map(&P.maps[0], g_pre, 8, (uint64_t)n, 256, DW_ROWS, l2) || tc_make_map(&P.maps[3], st_x, 8, (uint64_t)n, 256, DW_ROWS, l2) ||
+      (!trunk_only && (tc_make_map(&P.maps[1], g_f, 1, (uint64_t)n, 256, DW_ROWS, l2) ||
+                       tc_make_map(&P.maps[2], g_v, 1, (uint64_t)n, 128, DW_ROWS, l2) ||
+                       tc_make_map(&P.maps[4], st_f, 1, (uint64_t)n, 256, DW_ROWS, l2))))
     NM_FAIL(ctx, NM_ERR_CUDA, "nm_dw_gemm: cuTensorMapEncodeTiled failed");
   P.out = out;
   P.bias_out = bias_out;
@@ -160,17 +164,17 @@ int nm_impl_dw_gemm(nm_ctx* ctx, const __half* g_pre, const __half* g_f, const _
   const long long blocks = (n + DW_ROWS - 1) / DW_ROWS;
   int pairs[DW_ITEMS];
   {
-    const double wsum = 8 * 1024.0 + 768.0;
+    const double wsum = trunk_only ? 7 * 1024.0 : 8 * 1024.0 + 768.0;
     int used = 0;
-    for (int k = 0; k < DW_ITEMS; ++k) {
+    for (int k = 0; k < n_items; ++k) {
       pairs[k] = (int)(pairs_total * (k < 8 ? 1024.0 : 768.0) / wsum);
       if (pairs[k] < 1) pairs[k] = 1;
       used += pairs[k];
     }
-    for (int k = 0; used < pairs_total; k = (k + 1) % DW_ITEMS) { ++pairs[k]; ++used; }
+    for (int k = 0; used < pairs_total; k = (k + 1) % n_items) { ++pairs[k]; ++used; }
   }
   int w = 0;
-  for (int k = 0; k < DW_ITEMS; ++k) {
+  for (int k = 0; k < n_items; ++k) {
     for (int p = 0; p < pairs[k]; ++p, ++w) {
       DwWork& W = P.work[w];
       if (k < 7) { W.a_map = 0; W.a_plane = k + 1; W.b_map = 3; W.b_plane = k; W.m_rows = 256; }

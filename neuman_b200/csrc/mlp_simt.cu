@@ -17,6 +17,7 @@ struct SimtParams {
   const float* alpha_w; const float* alpha_b;
   const float* views_w; const float* views_b;
   const float* rgb_w; const float* rgb_b;
+  const float* out_w; const float* out_b;     // output_linear of a view-independent net: Wt [256][4], bias [4]
   NmPeSpec pos_pe, dir_pe;
 };
 
@@ -62,7 +63,10 @@ __device__ __forceinline__ void zero_acc(float (&acc)[8][NJ]) {
     for (int j = 0; j < NJ; ++j) acc[i][j] = 0.f;
 }
 
-__global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in, float* __restrict__ raw) {
+// kView: use_viewdirs=True (alpha, feature, views and rgb heads); otherwise output_linear on layer 7 (:145-146) and no
+// direction input
+template <bool kView>
+__device__ __forceinline__ void mlp_simt_body(const SimtParams& P, const NmMlpInput& in, float* __restrict__ raw) {
   extern __shared__ float sm[];
   float* hA = sm;                    // [64][256]
   float* hB = hA + TM * 256;         // [64][256]
@@ -73,7 +77,7 @@ __global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in,
   const long long base = (long long)blockIdx.x * TM;
 
   // ---- positional encodings ----
-  const int npos = 3 * P.pos_pe.n_freqs, ndir = 3 * P.dir_pe.n_freqs;
+  const int npos = 3 * P.pos_pe.n_freqs, ndir = kView ? 3 * P.dir_pe.n_freqs : 0;
   for (int t = tid; t < TM * (npos + ndir + 2); t += NT) {
     int s = t / (npos + ndir + 2), q = t - s * (npos + ndir + 2);
     long long i = base + s;
@@ -89,7 +93,7 @@ __global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in,
       vpe[s * 32 + ci] = sn; vpe[s * 32 + cj] = cs;
     } else if (q == npos + ndir) {
       pe[s * 64 + 0] = p[0]; pe[s * 64 + 1] = p[1]; pe[s * 64 + 2] = p[2]; pe[s * 64 + 63] = 0.f;
-    } else {
+    } else if (kView) {
       vpe[s * 32 + 0] = v[0]; vpe[s * 32 + 1] = v[1]; vpe[s * 32 + 2] = v[2];
 #pragma unroll
       for (int c = 27; c < 32; ++c) vpe[s * 32 + c] = 0.f;
@@ -118,6 +122,16 @@ __global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in,
     store_out<8>(acc, P.b[l], true, nxt, 256, tx, ty);
     __syncthreads();
     float* t = cur; cur = nxt; nxt = t;
+  }
+  if (!kView) {
+    // raw = output_linear(h7) (:146), fp32 FMAs over k in order, then the bias
+    const int s = tid >> 2, o = tid & 3;
+    const long long i = base + s;
+    const float* h = cur + (size_t)s * 256;
+    float a = 0.f;
+    for (int k = 0; k < 256; ++k) a = fmaf(h[k], __ldg(P.out_w + (size_t)k * 4 + o), a);
+    if (i < in.n) raw[4 * i + o] = a + __ldg(P.out_b + o);
+    return;
   }
   // alpha = alpha_linear(h7)   (:135)
   if (tid < TM) {
@@ -158,6 +172,13 @@ __global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in,
   }
 }
 
+__global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in, float* __restrict__ raw) {
+  mlp_simt_body<true>(P, in, raw);
+}
+__global__ void __launch_bounds__(NT, 1) k_mlp_simt_noview(SimtParams P, NmMlpInput in, float* __restrict__ raw) {
+  mlp_simt_body<false>(P, in, raw);
+}
+
 int nm_simt_forward(nm_ctx* ctx, const NmNet& net, const float* pts, const float* views, const float* origins,
                     const float* dirs, const float* z, int64_t n, int32_t group, float* raw, cudaStream_t st) {
   SimtParams P;
@@ -166,13 +187,19 @@ int nm_simt_forward(nm_ctx* ctx, const NmNet& net, const float* pts, const float
   P.alpha_w = net.f32 + net.o_alpha_w; P.alpha_b = net.f32 + net.o_alpha_b;
   P.views_w = net.f32 + net.o_views_w; P.views_b = net.f32 + net.o_views_b;
   P.rgb_w = net.f32 + net.o_rgb_w; P.rgb_b = net.f32 + net.o_rgb_b;
+  P.out_w = net.f32 + net.o_out_w; P.out_b = net.f32 + net.o_out_b;
   P.pos_pe = {net.desc.pos_pe_kind, net.desc.pos_n_freqs, net.f32 + net.o_pos_bv};
   P.dir_pe = {net.desc.dir_pe_kind, net.desc.dir_n_freqs, net.f32 + net.o_dir_bv};
   NmMlpInput in{pts, views, origins, dirs, z, (long long)n, group};
   size_t smem = (size_t)(2 * TM * 256 + TM * 64 + TM * 32 + TM) * sizeof(float);
-  NM_SET_SMEM_ONCE(ctx, (k_mlp_simt), (int)smem);
   unsigned blocks = (unsigned)((n + TM - 1) / TM);
-  k_mlp_simt<<<blocks, NT, smem, st>>>(P, in, raw);
+  if (net.kind == NM_NET_VIEW) {
+    NM_SET_SMEM_ONCE(ctx, (k_mlp_simt), (int)smem);
+    k_mlp_simt<<<blocks, NT, smem, st>>>(P, in, raw);
+  } else {
+    NM_SET_SMEM_ONCE(ctx, (k_mlp_simt_noview), (int)smem);
+    k_mlp_simt_noview<<<blocks, NT, smem, st>>>(P, in, raw);
+  }
   NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }

@@ -37,16 +37,22 @@ struct TcPlan {
 // get one extra k-block, a "bias slab" that is zero except for column 63, consumed by ONE K = 16 MMA against the last K
 // slice (channels 48..63) of the position encoding: channels 48..62 meet zero weights, channel 63 is 1.  The epilogue then
 // has no bias loads and no adds at all; the extra MMA costs 1/16 of a layer's tensor time.
-__host__ __device__ constexpr int step_nkb(int s) { return s == 0 ? 1 : (s == 10 ? 2 : 5); }
-__host__ __device__ constexpr bool kb_is_bias(int s, int kb) { return kb == 4 && s != 5 && s != 9 && s >= 1 && s <= 8; }
-__host__ __device__ constexpr int step_N(int s) { return s <= 8 ? 256 : (s == 9 ? 128 : 16); }
+// `v` selects the net kind: true = view-dependent (steps 0-10 above), false = view-independent (use_viewdirs=False,
+// models/vanilla.py:145-146): steps 0-7 as above, then step 8 = output_linear (N = 16, 4 used, K = 256 over the layer-7
+// activation block, :146); no alpha, feature, views or rgb step, no direction encoding.
+__host__ __device__ constexpr int tc_steps(bool v) { return v ? TC_STEPS : 9; }
+__host__ __device__ constexpr int step_nkb(int s, bool v = true) { return s == 0 ? 1 : (s == 10 ? 2 : (!v && s == 8 ? 4 : 5)); }
+__host__ __device__ constexpr bool kb_is_bias(int s, int kb, bool v = true) {
+  return kb == 4 && s != 5 && s != 9 && s >= 1 && (v ? s <= 8 : s <= 7);
+}
+__host__ __device__ constexpr int step_N(int s, bool v = true) { return s <= 7 || (v && s == 8) ? 256 : (v && s == 9 ? 128 : 16); }
 // k-block kb of step s reads the position encoding / the direction encoding (else activation block `act_kb`)
-__host__ __device__ constexpr bool kb_is_pos(int s, int kb) { return (s == 0) || (s == 5 && kb == 0) || kb_is_bias(s, kb); }
-__host__ __device__ constexpr bool kb_is_dir(int s, int kb) { return s == 9 && kb == 4; }
+__host__ __device__ constexpr bool kb_is_pos(int s, int kb, bool v = true) { return (s == 0) || (s == 5 && kb == 0) || kb_is_bias(s, kb, v); }
+__host__ __device__ constexpr bool kb_is_dir(int s, int kb, bool v = true) { return v && s == 9 && kb == 4; }
 __host__ __device__ constexpr int kb_act_index(int s, int kb) { return s == 5 ? kb - 1 : kb; }
-__host__ __device__ constexpr int tc_slabs_per_tile() {
+__host__ __device__ constexpr int tc_slabs_per_tile(bool v = true) {
   int n = 0;
-  for (int s = 0; s < TC_STEPS; ++s) n += step_nkb(s);
+  for (int s = 0; s < tc_steps(v); ++s) n += step_nkb(s, v);
   return n;
 }
 
@@ -65,6 +71,7 @@ struct TcCfg {
 static_assert(TcCfg::SMEM_BYTES <= 232448, "shared memory of the forward kernel exceeds 227 KB");
 
 // constant table of the epilogue: [0, 256) alpha_linear.weight | 256..258 rgb bias | 259 alpha bias
+// (view-independent nets: [0, 256) unused | 256..259 output_linear.bias)
 #define TC_CONST_ALPHA 0
 #define TC_CONST_OUT 256
 
@@ -80,10 +87,11 @@ struct TcParams {
   int range_phase;          // sampled range check: the rounds r with r % 64 == range_phase % 64 are checked
   // training forward (kTrain): fp16 activation stash for the backward pass, planes of n rows each
   __half* st_x;             // [8][n][256] post-ReLU outputs of layers 0..7
-  __half* st_f;             // [n][256]    feature_linear output
-  __half* st_v;             // [n][128]    views layer post-ReLU
+  __half* st_f;             // [n][256]    feature_linear output (view-dependent nets only)
+  __half* st_v;             // [n][128]    views layer post-ReLU (view-dependent nets only)
   uint32_t* st_m;           // [9][n][8]   sign words, 16 bits per 16 columns: bit j = [col 2j > 0], bit 8+j = [col 2j+1 > 0];
-                            //             planes 0..7 = pts_linears, plane 8 = views layer (words 0..3 used)
+                            //             planes 0..7 = pts_linears, plane 8 = views layer (words 0..3 used; view-independent
+                            //             nets: [8][n][8], no plane 8)
   CUtensorMap map_x, map_f, map_v;   // TMA store maps of st_x / st_f / st_v (kTrain only)
 };
 
@@ -219,12 +227,14 @@ __device__ __forceinline__ void quad_or(uint32_t (&w)[8]) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// The kernel
+// The kernel body, shared by the view-dependent (kView) and view-independent nets: same tile loop, same ring, same steps 0-7
 // ---------------------------------------------------------------------------------------------
-template <bool kTrain>
-__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
+template <bool kTrain, bool kView>
+__device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
   using C = TcCfg;
-  constexpr int SLABS = tc_slabs_per_tile();
+  constexpr int SLABS = tc_slabs_per_tile(kView);
+  constexpr int STEPS = tc_steps(kView);
+  constexpr int LAST = STEPS - 1;                       // the output step: rgb (N = 16) or output_linear (N = 16)
   extern __shared__ uint8_t smem_dyn[];
   const uint32_t pad = (1024 - (smem_u32(smem_dyn) & 1023)) & 1023;     // SWIZZLE_128B atoms: 1024-byte aligned base
   uint8_t* smem = smem_dyn + pad;
@@ -250,7 +260,7 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
     mbar_arrive_expect_tx(R.full(pq), bytes);
     bulk_g2s(R.slot(pq), P.wimg + P.plan.slab_off[ps][pkb], bytes, R.full(pq));
     ++pq;
-    if (++pkb == step_nkb(ps)) { pkb = 0; if (++ps == TC_STEPS) ps = 0; }
+    if (++pkb == step_nkb(ps, kView)) { pkb = 0; if (++ps == STEPS) ps = 0; }
   };
   if (threadIdx.x == 0) {
     R.init();
@@ -272,7 +282,9 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
   for (long long it = 0; it < my_tiles; ++it) {
     const long long tile = blockIdx.x + it * gridDim.x;
     const long long row0 = tile * 128 + wg * TC_WG_ROWS;          // first sample of this warpgroup
-    const bool track = (it % rperiod) == (P.range_phase % rperiod);
+    // view-independent nets check every tile: with the sampled (data-dependent) check ptxas serialises the wgmma of their
+    // training variant (C7520); the epilogue has the ALU time to spare without the alpha head
+    const bool track = !kView || (it % rperiod) == (P.range_phase % rperiod);
     // ---- encodings (Embedder.forward, models/vanilla.py:82-92): threads 0-63 position, 64-127 direction of row wtid % 64 ----
     {
       // Ray / view row of sample row0 + r: one 64-bit division per tile, then a 32-bit one per thread.  A per-thread
@@ -291,33 +303,33 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
       if (wtid < 64) {
         encode_f16(P.pos_pe, p, e, 30);
         store_row_swizzled(wbuf + C::OFF_POS, r, e, 8);
-      } else {
+      } else if (kView) {
         encode_f16(P.dir_pe, v, e, 12);
         store_row_swizzled(wbuf + C::OFF_DIR, r, e, 4);
       }
-      if (track) { track_range<false>(rng, e[0]); track_range<false>(rng, e[1]); }   // raw x, y, z (+ one sine)
+      if (track && (kView || wtid < 64)) { track_range<false>(rng, e[0]); track_range<false>(rng, e[1]); }   // raw x, y, z (+ one sine)
       fence_async_smem();
       wg_sync(wg);
     }
     float alpha[2] = {0.f, 0.f};
-    for (int s = 0; s < TC_STEPS; ++s) {
-      const int nkb = step_nkb(s);
+    for (int s = 0; s < STEPS; ++s) {
+      const int nkb = step_nkb(s, kView);
       wgmma_fence();
       for (int kb = 0; kb < nkb; ++kb) {
         const uint32_t qq = qbase + kb;
         R.wait_full(qq);
-        const uint32_t a_addr = kb_is_pos(s, kb) ? wbase + C::OFF_POS
-                              : kb_is_dir(s, kb) ? wbase + C::OFF_DIR
+        const uint32_t a_addr = kb_is_pos(s, kb, kView) ? wbase + C::OFF_POS
+                              : kb_is_dir(s, kb, kView) ? wbase + C::OFF_DIR
                                                  : wbase + kb_act_index(s, kb) * TC_KB_BYTES;
         // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
         // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab)
-        const bool bias = kb_is_bias(s, kb);
-        const int k0 = bias ? 3 : 0, k1 = kb_is_dir(s, kb) ? 2 : 4;
+        const bool bias = kb_is_bias(s, kb, kView);
+        const int k0 = bias ? 3 : 0, k1 = kb_is_dir(s, kb, kView) ? 2 : 4;
         const uint64_t a_desc = gmma_desc_k(a_addr), b_desc = gmma_desc_k(R.slot(qq));
         for (int k = k0; k < k1; ++k) {
           const uint32_t acc = (kb | (k - k0)) != 0;
-          if (s <= 8) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
-          else if (s == 9) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+          if (s <= (kView ? 8 : 7)) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+          else if (kView && s == 9) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
           else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
         }
         wgmma_commit();
@@ -328,30 +340,30 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
       wgmma_fence_regs(d16);
       release(qbase + nkb - 1);
       qbase += nkb;
-      if (s < 10) {
+      if (s < LAST) {
         // the MMAs of this step read the activation buffer, the stash stores of the previous step still may: both must
         // be done before the epilogue overwrites it
         if (kTrain && wtid == 0) tma_store_wait_read();
         wg_sync(wg);
         uint32_t wA[8] = {0, 0, 0, 0, 0, 0, 0, 0}, wB[8] = {0, 0, 0, 0, 0, 0, 0, 0};
         const float* s_walpha = s_const + TC_CONST_ALPHA;
-        if (s == 7) fwd_epi<256, true, true, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
-        else if (s == 8) fwd_epi<256, false, false, false>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        if (s == 7) fwd_epi<256, true, kView, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else if (kView && s == 8) fwd_epi<256, false, false, false>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
         else if (s == 9) fwd_epi<128, true, false, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
         else fwd_epi<256, true, false, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
         fence_async_smem();
         wg_sync(wg);
         if (kTrain) {
           if (wtid == 0) {
-            if (s < 8) tma_store_rows(&P.map_x, wbase, 0, 4, row0, s);
+            if (!kView || s < 8) tma_store_rows(&P.map_x, wbase, 0, 4, row0, s);
             else if (s == 8) tma_store_rows(&P.map_f, wbase, 0, 4, row0, 0);
             else tma_store_rows(&P.map_v, wbase, 0, 2, row0, 0);
           }
-          if (s != 8) {
+          if (!kView || s != 8) {
             quad_or(wA);
             quad_or(wB);
             const long long iA = row0 + rA, iB = iA + 8;
-            if (s < 8) {
+            if (!kView || s < 8) {
               uint32_t* m = P.st_m + (size_t)s * P.in.n * 8;
               if (iA < P.in.n) reinterpret_cast<uint2*>(m + iA * 8)[q] = make_uint2(wA[2 * q], wA[2 * q + 1]);
               if (iB < P.in.n) reinterpret_cast<uint2*>(m + iB * 8)[q] = make_uint2(wB[2 * q], wB[2 * q + 1]);
@@ -362,14 +374,14 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
             }
           }
         }
-        if (s == 7) {
+        if (kView && s == 7) {
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
             alpha[r] += __shfl_xor_sync(0xffffffffu, alpha[r], 1);
             alpha[r] += __shfl_xor_sync(0xffffffffu, alpha[r], 2);
           }
         }
-      } else {
+      } else if (kView) {
         // rgb (columns 0..2: lane q = 0 holds 0, 1; lane q = 1 holds 2) and the alpha head -> raw [r, g, b, sigma] (:144)
         const float bA = __shfl_down_sync(0xffffffffu, d16[0], 1), bB = __shfl_down_sync(0xffffffffu, d16[2], 1);
         const long long iA = row0 + rA, iB = iA + 8;
@@ -377,11 +389,31 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
           reinterpret_cast<float4*>(P.raw)[iA] = make_float4(d16[0] + ob.x, d16[1] + ob.y, bA + ob.z, alpha[0] + ob.w);
         if (q == 0 && iB < P.in.n)
           reinterpret_cast<float4*>(P.raw)[iB] = make_float4(d16[2] + ob.x, d16[3] + ob.y, bB + ob.z, alpha[1] + ob.w);
+      } else {
+        // output_linear (:146): columns 0..3 = raw [r, g, b, sigma]; lane q = 0 holds 0, 1, lane q = 1 holds 2, 3
+        const float cA = __shfl_down_sync(0xffffffffu, d16[0], 1), dA = __shfl_down_sync(0xffffffffu, d16[1], 1);
+        const float cB = __shfl_down_sync(0xffffffffu, d16[2], 1), dB = __shfl_down_sync(0xffffffffu, d16[3], 1);
+        const long long iA = row0 + rA, iB = iA + 8;
+        if (q == 0 && iA < P.in.n)
+          reinterpret_cast<float4*>(P.raw)[iA] = make_float4(d16[0] + ob.x, d16[1] + ob.y, cA + ob.z, dA + ob.w);
+        if (q == 0 && iB < P.in.n)
+          reinterpret_cast<float4*>(P.raw)[iB] = make_float4(d16[2] + ob.x, d16[3] + ob.y, cB + ob.z, dB + ob.w);
       }
     }
   }
   if (((rng & 0xFFFFu) >= 0x7BFFu) || ((rng >> 16) >= 0x7BFFu)) atomicOr(P.range_flag, 1);
   if (kTrain && wtid == 0) tma_store_wait_all();
+}
+
+// view-dependent nets (use_viewdirs=True): render (kTrain = false) and training forward
+template <bool kTrain>
+__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
+  mlp_tc_body<kTrain, true>(P);
+}
+// view-independent nets (use_viewdirs=False): no direction input, output_linear head
+template <bool kTrain>
+__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc_noview(const __grid_constant__ TcParams P) {
+  mlp_tc_body<kTrain, false>(P);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -390,11 +422,13 @@ __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_const
 struct PackSrc {
   const float* w[8]; const float* feat; const float* views; const float* rgb;
   const float* b[8]; const float* feat_b; const float* views_b;      // biases: they ride in the slabs (column of the constant-1 channel)
+  const float* out_t;                                                 // output_linear.weight as [256][4] (view-independent nets)
 };
 
-// weight of (step s, output n, k-block kb, kk in [0,64)) or 0 for padding
-__device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int kb, int kk) {
-  if (kb_is_bias(s, kb)) {                       // bias slab of a K = 256 step: only the column of PE channel 63 is non-zero
+// weight of (step s, output n, k-block kb, kk in [0,64)) or 0 for padding; `view` = the net kind (step tables above)
+__device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int kb, int kk, bool view) {
+  if (!view && s == 8) return n < 4 ? S.out_t[(size_t)(kb * 64 + kk) * 4 + n] : 0.f;   // output_linear, N padded 4 -> 16
+  if (kb_is_bias(s, kb, view)) {                 // bias slab of a K = 256 step: only the column of PE channel 63 is non-zero
     if (kk != 63) return 0.f;
     return s == 8 ? S.feat_b[n] : S.b[s][n];
   }
@@ -415,22 +449,22 @@ __device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int 
   return n < 3 ? S.rgb[(size_t)n * 128 + kb * 64 + kk] : 0.f;
 }
 
-__global__ void k_tc_pack(PackSrc S, TcPlan plan, __half* __restrict__ out) {
+__global__ void k_tc_pack(PackSrc S, TcPlan plan, bool view, __half* __restrict__ out) {
   // one thread per packed element of the image
   const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;      // half index inside the image
   if (e * 2 >= plan.image_bytes) return;
   const uint32_t byte = (uint32_t)(e * 2);
   // locate (s, kb)
   int s = 0, kb = 0;
-  for (int ss = 0; ss < TC_STEPS; ++ss)
-    for (int k = 0; k < step_nkb(ss); ++k)
+  for (int ss = 0; ss < tc_steps(view); ++ss)
+    for (int k = 0; k < step_nkb(ss, view); ++k)
       if (byte >= plan.slab_off[ss][k]) { s = ss; kb = k; }
   const uint32_t in_slab = byte - plan.slab_off[s][kb];
   const int n = in_slab >> 7;
   const int chunk_phys = (in_slab & 127) >> 4;
   const int chunk = chunk_phys ^ (n & 7);                               // undo the 128B swizzle
   const int kk = chunk * 8 + ((in_slab & 15) >> 1);
-  out[e] = __float2half_rn(src_weight(S, s, n, kb, kk));
+  out[e] = __float2half_rn(src_weight(S, s, n, kb, kk, view));
 }
 
 // the constant table of the epilogue (layout: TC_CONST_ALPHA / TC_CONST_OUT)
@@ -438,6 +472,12 @@ __global__ void k_tc_consts(const float* rgb_b, const float* alpha_w, const floa
   const int i = threadIdx.x;      // 256 threads
   out[TC_CONST_ALPHA + i] = alpha_w[i];
   if (i < TC_CONST_FLOATS - TC_CONST_OUT) out[TC_CONST_OUT + i] = i < 3 ? rgb_b[i] : (i == 3 ? alpha_b[0] : 0.f);
+}
+// ... of a view-independent net: no alpha weights, output_linear.bias at TC_CONST_OUT
+__global__ void k_tc_consts_noview(const float* out_b, float* __restrict__ out) {
+  const int i = threadIdx.x;      // 256 threads
+  out[TC_CONST_ALPHA + i] = 0.f;
+  if (i < TC_CONST_FLOATS - TC_CONST_OUT) out[TC_CONST_OUT + i] = i < 4 ? out_b[i] : 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -476,19 +516,20 @@ int nm_tc_encode(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64
   return NM_OK;
 }
 
-static TcPlan make_plan() {
+static TcPlan make_plan(bool view) {
   TcPlan p{};
   uint32_t off = 0;
-  for (int s = 0; s < TC_STEPS; ++s) {
-    p.slab_bytes[s] = (uint32_t)step_N(s) * 128u;
-    for (int kb = 0; kb < step_nkb(s); ++kb) { p.slab_off[s][kb] = off; off += p.slab_bytes[s]; }
+  for (int s = 0; s < tc_steps(view); ++s) {
+    p.slab_bytes[s] = (uint32_t)step_N(s, view) * 128u;
+    for (int kb = 0; kb < step_nkb(s, view); ++kb) { p.slab_off[s][kb] = off; off += p.slab_bytes[s]; }
   }
   p.image_bytes = off;
   return p;
 }
 
 int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
-  TcPlan plan = make_plan();
+  const bool view = net.kind == NM_NET_VIEW;
+  TcPlan plan = make_plan(view);
   const size_t halfs = plan.image_bytes / 2;
   if (!net.f16 || net.f16_halfs != halfs) {
     if (net.f16) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(net.f16)); net.f16 = nullptr; }
@@ -502,19 +543,22 @@ int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   S.feat = d.feature_w; S.views = d.views_w; S.rgb = d.rgb_w;
   for (int l = 0; l < 8; ++l) S.b[l] = d.pts_b[l];
   S.feat_b = d.feature_b; S.views_b = d.views_b;
-  k_tc_pack<<<(unsigned)((halfs + 255) / 256), 256, 0, st>>>(S, plan, net.f16);
+  S.out_t = net.f32 + net.o_out_w;
+  k_tc_pack<<<(unsigned)((halfs + 255) / 256), 256, 0, st>>>(S, plan, view, net.f16);
   NM_CHECK_LAUNCH(ctx);
-  k_tc_consts<<<1, 256, 0, st>>>(d.rgb_b, d.alpha_w, d.alpha_b, net.tc_bias);
+  if (view) k_tc_consts<<<1, 256, 0, st>>>(d.rgb_b, d.alpha_w, d.alpha_b, net.tc_bias);
+  else k_tc_consts_noview<<<1, 256, 0, st>>>(net.f32 + net.o_out_b, net.tc_bias);
   NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }
 
-template <bool kTrain>
+template <bool kTrain, bool kView>
 static int launch_tc(nm_ctx* ctx, const TcParams& P, cudaStream_t st) {
-  NM_SET_SMEM_ONCE(ctx, k_mlp_tc<kTrain>, TcCfg::SMEM_BYTES);
+  auto kernel = kView ? k_mlp_tc<kTrain> : k_mlp_tc_noview<kTrain>;
+  NM_SET_SMEM_ONCE(ctx, kernel, TcCfg::SMEM_BYTES);
   long long ctas = ctx->sm_count;
   if (P.n_tiles < ctas) ctas = P.n_tiles > 0 ? P.n_tiles : 1;
-  k_mlp_tc<kTrain><<<(unsigned)ctas, TcCfg::THREADS, TcCfg::SMEM_BYTES, st>>>(P);
+  kernel<<<(unsigned)ctas, TcCfg::THREADS, TcCfg::SMEM_BYTES, st>>>(P);
   NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }
@@ -523,9 +567,10 @@ int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
                   const float* dirs, const float* z, int64_t n, int32_t group, float* raw, cudaStream_t st,
                   const NmTrainStash* stash) {
   if (!net.f16 || !net.tc_bias) NM_FAIL(ctx, NM_ERR_STATE, "nm_tc_forward: weights not packed");
+  const bool view = net.kind == NM_NET_VIEW;
   TcParams P;
   P.wimg = reinterpret_cast<const uint8_t*>(net.f16);
-  P.plan = make_plan();
+  P.plan = make_plan(view);
   P.in = NmMlpInput{pts, views, origins, dirs, z, (long long)n, group};
   P.pos_pe = NmPeSpec{net.desc.pos_pe_kind, net.desc.pos_n_freqs, net.f32 + net.o_pos_cyc};
   P.dir_pe = NmPeSpec{net.desc.dir_pe_kind, net.desc.dir_n_freqs, net.f32 + net.o_dir_cyc};
@@ -539,9 +584,10 @@ int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
   memset(&P.map_x, 0, 3 * sizeof(CUtensorMap));
   if (stash) {
     if (n >= (int64_t)0x7fff0000) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_train: n too large for one call");
-    if (tc_make_store_map(&P.map_x, stash->x, 8, (uint64_t)n, 256) || tc_make_store_map(&P.map_f, stash->f, 1, (uint64_t)n, 256) ||
-        tc_make_store_map(&P.map_v, stash->v, 1, (uint64_t)n, 128))
+    if (tc_make_store_map(&P.map_x, stash->x, 8, (uint64_t)n, 256) ||
+        (view && (tc_make_store_map(&P.map_f, stash->f, 1, (uint64_t)n, 256) || tc_make_store_map(&P.map_v, stash->v, 1, (uint64_t)n, 128))))
       NM_FAIL(ctx, NM_ERR_CUDA, "nm_mlp_forward_train: cuTensorMapEncodeTiled failed");
   }
-  return stash ? launch_tc<true>(ctx, P, st) : launch_tc<false>(ctx, P, st);
+  if (!view) return stash ? launch_tc<true, false>(ctx, P, st) : launch_tc<false, false>(ctx, P, st);
+  return stash ? launch_tc<true, true>(ctx, P, st) : launch_tc<false, true>(ctx, P, st);
 }

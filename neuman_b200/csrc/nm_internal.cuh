@@ -17,23 +17,31 @@
 #define NM_RANGE_FLAG_WORD 32  // word of ctx->d_counter the tensor-core kernels OR their range flag into
 
 // ---- packed network ------------------------------------------------------------------------
+// Net kinds: NeRF with use_viewdirs=True (alpha / feature / views / rgb heads, nm_net_pack) or use_viewdirs=False
+// (one output_linear [4,256] on layer 7, no direction input, nm_net_pack_noview; models/vanilla.py:117-118,145-146).
+enum { NM_NET_VIEW = 0, NM_NET_NOVIEW = 1 };
+
 // fp32 transposed weights ([in_padded][out]) for the SIMT kernel live in one device allocation per slot; the
 // tensor-core kernels read fp16 slabs in the 128B-swizzled wgmma layout from their own allocations.
 struct NmNet {
   bool packed = false;
-  nm_nerf_desc desc{};
+  int kind = NM_NET_VIEW;
+  nm_nerf_desc desc{};              // view-independent nets: the trunk and position-encoding fields; head pointers null
   // SIMT fp32 layout: Wt[k][n] (k = input index, n = output index), biases as given
   float* f32 = nullptr;             // base allocation
   size_t f32_floats = 0;
   // offsets (in floats) into f32
   size_t o_pts_w[8], o_pts_b[8], o_feat_w, o_feat_b, o_alpha_w, o_alpha_b, o_views_w, o_views_b,
-      o_rgb_w, o_rgb_b, o_pos_bv, o_dir_bv, o_pos_cyc, o_dir_cyc;
+      o_rgb_w, o_rgb_b, o_pos_bv, o_dir_bv, o_pos_cyc, o_dir_cyc,
+      o_out_w, o_out_b;             // output_linear of a view-independent net: Wt [256][4], bias [4]
   // tensor-core layout (see mlp_tc.cu for the tile format)
   __half* f16 = nullptr;
   size_t f16_halfs = 0;
   float* tc_bias = nullptr;         // epilogue constants: alpha weights, output biases (mlp_tc.cu k_tc_consts)
   __half* f16_bwd = nullptr;        // transposed slabs for the backward chain (mlp_tc_bwd.cu), packed on first use
-  float* bw_wrgb = nullptr;         // rgb_linear.weight as [3][128] for the backward kernel's constant bank
+  float* bw_wrgb = nullptr;         // backward kernel's constant bank: rgb_linear.weight as [3][128] (view-independent
+                                    // nets: output_linear.weight as [4][256])
+  size_t bwd_bytes = 0, bw_wrgb_floats = 0;   // sizes of the two, which depend on the kind
   bool bwd_packed = false;
   nm_nerf_desc pe_desc{};           // description the uploaded encoding tables were built from
   bool pe_valid = false;
@@ -188,9 +196,10 @@ int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st);
 // fp16 activation stash written by the training forward and read by the backward chain (mlp_tc_bwd.cu)
 struct NmTrainStash {
   __half* x;     // [8][n][256] post-ReLU outputs of pts_linears 0..7
-  __half* f;     // [n][256]    feature_linear output
-  __half* v;     // [n][128]    views layer post-ReLU
-  uint32_t* m;   // [9][n][8]   ReLU sign words: planes 0..7 pts_linears, plane 8 views layer (16 bits per 16 columns, mlp_tc.cu fwd_epi)
+  __half* f;     // [n][256]    feature_linear output (null for view-independent nets)
+  __half* v;     // [n][128]    views layer post-ReLU (null for view-independent nets)
+  uint32_t* m;   // [9][n][8]   ReLU sign words: planes 0..7 pts_linears, plane 8 views layer (16 bits per 16 columns, mlp_tc.cu fwd_epi);
+                 //             view-independent nets: [8][n][8]
 };
 int nm_impl_pe_backward(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64_t group, const float* d_enc, int ld,
                         const float* inv_scale, int64_t n, float* d_x, cudaStream_t st);

@@ -36,10 +36,20 @@ def _originals(mod, names):
 
 
 def supported_joiner(j):
-    """True when `j` is a Joiner the kernels implement: 8x256 trunk, skip after layer 4, view directions, no output
-    scaling, 10 / 4 log-spaced frequencies with the input included, 'posenc' or 'rotate' mapping."""
+    """True when `j` is a Joiner the kernels implement: 8x256 trunk, skip after layer 4, no output scaling, 10
+    log-spaced position frequencies with the input included, 'posenc' or 'rotate' mapping, and either view directions
+    (4 direction frequencies, same conditions) or no view directions with output_linear [4,256] (use_viewdirs=False:
+    the direction encoding is never used)."""
     try:
-        n, pp, dp = j.nerf, j.pos_pe, j.dir_pe
+        n, pp = j.nerf, j.pos_pe
+        if not n.use_viewdirs:
+            return bool(len(n.pts_linears) == 8 and tuple(n.skips) == (4,)
+                        and tuple(n.pts_linears[1].weight.shape) == (256, 256)
+                        and tuple(n.output_linear.weight.shape) == (4, 256)
+                        and getattr(n, "scale_type", "no") == "no"
+                        and pp.N_freqs == 10 and pp.input_dims == 3 and pp.log_sampling and pp.include_input
+                        and pp.mapping in ("posenc", "rotate"))
+        dp = j.dir_pe
         return bool(n.use_viewdirs and len(n.pts_linears) == 8 and tuple(n.skips) == (4,)
                     and tuple(n.pts_linears[1].weight.shape) == (256, 256)
                     and getattr(n, "scale_type", "no") == "no"
@@ -81,7 +91,9 @@ def install(reference_root=None, train=False):
     ref_forward = o_joiner["forward"]
 
     def joiner_forward(self, input_pts, input_views=None):
-        if input_views is not None and on_cuda(input_pts, input_views) and supported_joiner(self):
+        viewless = not getattr(self.nerf, "use_viewdirs", True)
+        if ((viewless and on_cuda(input_pts)) or (input_views is not None and on_cuda(input_pts, input_views))) \
+                and supported_joiner(self):
             if not torch.is_grad_enabled():
                 return ops.joiner_forward(self, input_pts, input_views)
             if train:

@@ -122,10 +122,11 @@ class Joiner(nn.Module):
         self.pos_pe, self.dir_pe, self.nerf = pos_pe, dir_pe, nerf
 
     def forward(self, input_pts, input_views=None):
-        """input_pts [...,3], input_views [...,3] -> [...,4] = (r,g,b,sigma). CUDA only.
+        """input_pts [...,3], input_views [...,3] -> [...,4] = (r,g,b,sigma). CUDA only.  A view-independent net
+        (use_viewdirs=False) ignores input_views, which may be None.
         Under autograd (a network parameter or an input requiring grad) the training kernel runs and the result
         carries gradients to the parameters and to input_pts / input_views (neuman_b200/autograd.py)."""
-        if torch.is_grad_enabled() and input_views is not None and (
+        if torch.is_grad_enabled() and (input_views is not None or not self.nerf.use_viewdirs) and (
                 any(p.requires_grad for p in self.nerf.parameters())
                 or any(isinstance(t, torch.Tensor) and t.requires_grad for t in (input_pts, input_views))):
             from . import autograd

@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import Context, NmCamera, NmNerfDesc, NM_MAX_ACTORS
+from ._lib import Context, NmCamera, NmNerfDesc, NmNerfNoviewDesc, NM_MAX_ACTORS
 
 DEFAULT_GEO_THRESH = 0.2     # utils/constant.py:14
 
@@ -85,8 +85,15 @@ def invalidate_net(joiner):
             _evict_uid(weakref.ref(ctx), tag[0])
 
 
+def is_viewless(joiner):
+    """True for a view-independent net (NeRF with use_viewdirs=False: one output_linear head, no direction input)."""
+    return not getattr(joiner.nerf, "use_viewdirs", True)
+
+
 def net_slot(joiner, ctx=None):
-    """Packs (lazily, keyed on a per-module uid + parameter storage + version) a Joiner into a library slot."""
+    """Packs (lazily, keyed on a per-module uid + parameter storage + version) a Joiner into a library slot: a
+    view-dependent net (use_viewdirs=True) with nm_net_pack, a view-independent one (use_viewdirs=False, output_linear
+    [4,256]) with nm_net_pack_noview."""
     nerf = joiner.nerf
     p0 = nerf.pts_linears[0].weight
     ctx = ctx or _ctx_for(p0)
@@ -96,8 +103,11 @@ def net_slot(joiner, ctx=None):
         ctx.slot_clock += 1
         ctx.slot_used[s] = ctx.slot_clock
         return s
-    if not getattr(nerf, "use_viewdirs", True):
-        raise NotImplementedError("only use_viewdirs=True networks are built (reference default)")
+    viewless = is_viewless(joiner)
+    if viewless and tuple(nerf.output_linear.weight.shape) != (4, 256):
+        raise NotImplementedError("view-independent nets: only output_linear [4,256] (output_ch=4) is built")
+    if viewless and getattr(nerf, "scale_type", "no") != "no":
+        raise NotImplementedError("view-independent nets: only scale_type='no' is built")
     if len(nerf.pts_linears) != 8 or nerf.pts_linears[1].weight.shape != (256, 256) or tuple(nerf.skips) != (4,):
         raise NotImplementedError("only the 8x256, skips=[4] architecture is built (reference default)")
     # stale entries of the same module
@@ -112,7 +122,7 @@ def net_slot(joiner, ctx=None):
     else:
         s = int(np.argmin(ctx.slot_used))
         ctx.slots.pop(ctx.slot_keys[s], None)
-    d = NmNerfDesc()
+    d = NmNerfNoviewDesc() if viewless else NmNerfDesc()
     keep = []
 
     def dev(t):
@@ -123,15 +133,21 @@ def net_slot(joiner, ctx=None):
     for i in range(8):
         d.pts_w[i] = dev(nerf.pts_linears[i].weight)
         d.pts_b[i] = dev(nerf.pts_linears[i].bias)
-    d.feature_w, d.feature_b = dev(nerf.feature_linear.weight), dev(nerf.feature_linear.bias)
-    d.alpha_w, d.alpha_b = dev(nerf.alpha_linear.weight), dev(nerf.alpha_linear.bias)
-    d.views_w, d.views_b = dev(nerf.views_linears[0].weight), dev(nerf.views_linears[0].bias)
-    d.rgb_w, d.rgb_b = dev(nerf.rgb_linear.weight), dev(nerf.rgb_linear.bias)
-    pp, dp = joiner.pos_pe, joiner.dir_pe
-    d.pos_pe_kind, d.dir_pe_kind = _PE_KIND[pp.mapping], _PE_KIND[dp.mapping]
+    pp = joiner.pos_pe
+    d.pos_pe_kind = _PE_KIND[pp.mapping]
     d.pos_min_freq, d.pos_max_freq, d.pos_n_freqs = float(pp.min_freq), float(pp.max_freq), int(pp.N_freqs)
-    d.dir_min_freq, d.dir_max_freq, d.dir_n_freqs = float(dp.min_freq), float(dp.max_freq), int(dp.N_freqs)
-    ctx.check(ctx.lib.nm_net_pack(ctx.h, s, C.byref(d), ctx.stream()))
+    if viewless:
+        d.output_w, d.output_b = dev(nerf.output_linear.weight), dev(nerf.output_linear.bias)
+        ctx.check(ctx.lib.nm_net_pack_noview(ctx.h, s, C.byref(d), ctx.stream()))
+    else:
+        d.feature_w, d.feature_b = dev(nerf.feature_linear.weight), dev(nerf.feature_linear.bias)
+        d.alpha_w, d.alpha_b = dev(nerf.alpha_linear.weight), dev(nerf.alpha_linear.bias)
+        d.views_w, d.views_b = dev(nerf.views_linears[0].weight), dev(nerf.views_linears[0].bias)
+        d.rgb_w, d.rgb_b = dev(nerf.rgb_linear.weight), dev(nerf.rgb_linear.bias)
+        dp = joiner.dir_pe
+        d.dir_pe_kind = _PE_KIND[dp.mapping]
+        d.dir_min_freq, d.dir_max_freq, d.dir_n_freqs = float(dp.min_freq), float(dp.max_freq), int(dp.N_freqs)
+        ctx.check(ctx.lib.nm_net_pack(ctx.h, s, C.byref(d), ctx.stream()))
     if keep:
         torch.cuda.current_stream(ctx.device).synchronize()  # `keep` temporaries may be freed after this
     ctx.slots[key] = s
@@ -142,15 +158,19 @@ def net_slot(joiner, ctx=None):
 
 
 def joiner_forward(joiner, input_pts, input_views=None, mode=None):
-    """Joiner.forward (models/vanilla.py:162-166) -> [...,4]."""
-    if input_views is None:
+    """Joiner.forward (models/vanilla.py:162-166) -> [...,4].  A view-independent net ignores input_views (may be None),
+    as the reference does (:145-146)."""
+    viewless = is_viewless(joiner)
+    if input_views is None and not viewless:
         raise NotImplementedError("use_viewdirs=True networks need input_views")
     ctx = _ctx_for(input_pts)
     slot = net_slot(joiner, ctx)
     shape = input_pts.shape[:-1]
     pts = _f32(input_pts).reshape(-1, 3)
-    views = _f32(input_views, pts.device).reshape(-1, 3)
-    assert views.shape[0] == pts.shape[0], "input_views must match input_pts"
+    views = None
+    if not viewless:
+        views = _f32(input_views, pts.device).reshape(-1, 3)
+        assert views.shape[0] == pts.shape[0], "input_views must match input_pts"
     raw = torch.empty(pts.shape[0], 4, device=pts.device, dtype=torch.float32)
     ctx.check(ctx.lib.nm_mlp_forward(ctx.h, slot, _mlp_mode() if mode is None else mode, _p(pts), _p(views),
                                      pts.shape[0], 0, _p(raw), ctx.stream()))
