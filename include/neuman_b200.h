@@ -175,6 +175,11 @@ int nm_near_far(nm_ctx* ctx, const float* origins, const float* dirs, int64_t R,
                 const float* verts, int32_t n_verts, float geo_threshold,
                 float* near_out, float* far_out, void* stream);
 
+/* The same near/far against the mesh of `actor` set by nm_mesh_set, as the frame drivers compute it: vertex groups of 32
+ * with a bounding sphere each, culled conservatively per ray, so the result equals the exhaustive loop's. */
+int nm_near_far_mesh(nm_ctx* ctx, int actor, const float* origins, const float* dirs, int64_t R, float geo_threshold,
+                     float* near_out, float* far_out, void* stream);
+
 /* ray_to_samples (utils/ray_utils.py:96-135). near/far: [R] or NULL with the scalar fallback;
  * t_rand: [R,S] uniforms for perturb>0 (clipped to [0.01,0.99] inside, :121-125) or NULL.
  * pts/dirs may be NULL when only z is wanted. */

@@ -71,6 +71,7 @@ SIGNATURES = {
     "nm_mlp_forward_rays": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _I64, _I32, _P, _P]),
     "nm_raygen": (C.c_int, [_P, C.POINTER(NmCamera), C.c_int, _I64, _I64, _P, _P, _P, _P]),
     "nm_near_far": (C.c_int, [_P, _P, _P, _I64, _P, _I32, _F, _P, _P, _P]),
+    "nm_near_far_mesh": (C.c_int, [_P, C.c_int, _P, _P, _I64, _F, _P, _P, _P]),
     "nm_ray_to_samples": (C.c_int, [_P, _P, _P, _P, _P, _F, _F, _I64, _I32, _I32, _P, _P, _P, _P, _P]),
     "nm_sample_pdf": (C.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _P, _P]),
     "nm_importance_samples": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _P, _P, _P, _P]),

@@ -251,7 +251,11 @@ __global__ void __launch_bounds__(256) k_raw2outputs_bwd(
       float t = __shfl_down_sync(FULL, inc, o);
       if (lane + o < 32) inc += t;
     }
-    float Q = tail + (inc - gw);                      // exclusive: elements after s
+    // exclusive (elements after s) as the next lane's inclusive sum, never inc - gw: behind an opaque sample Q is tiny next
+    // to its own G*w, and the subtraction would leave only the rounding error of inc
+    float exc = __shfl_down_sync(FULL, inc, 1);
+    if (lane == 31) exc = 0.f;
+    float Q = tail + exc;
     tail += __shfl_sync(FULL, inc, 0);
     if (live) {
       float4 v = rr[s];

@@ -360,6 +360,15 @@ int nm_impl_near_far_mesh(nm_ctx* ctx, const NmMesh& m, const float* origins, co
   return NM_OK;
 }
 
+extern "C" int nm_near_far_mesh(nm_ctx* ctx, int actor, const float* origins, const float* dirs, int64_t R,
+                                float geo_threshold, float* near_out, float* far_out, void* stream) {
+  NM_ENTER(ctx);
+  if (R == 0) return NM_OK;
+  if (!origins || !dirs || !near_out || !far_out || R < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_near_far_mesh: bad argument");
+  if (actor < 0 || actor >= NM_MAX_ACTORS || !ctx->meshes[actor].set) NM_FAIL(ctx, NM_ERR_STATE, "nm_near_far_mesh: mesh not set");
+  return nm_impl_near_far_mesh(ctx, ctx->meshes[actor], origins, dirs, R, geo_threshold, near_out, far_out, (cudaStream_t)stream);
+}
+
 // ---------------------------------------------------------------------------------------------
 // ray_to_samples: thread per sample (coalesced along the sample index).
 __global__ void __launch_bounds__(256) k_ray_to_samples(

@@ -249,6 +249,18 @@ def geometry_guided_near_far(orig, dir, vert, geo_threshold=DEFAULT_GEO_THRESH):
     return near, far
 
 
+def near_far_mesh(orig, dir, actor, geo_threshold=DEFAULT_GEO_THRESH):
+    """geometry_guided_near_far against the mesh of `actor` (set_mesh), computed as the frame drivers do."""
+    ctx = _ctx_for(orig)
+    o, d = _f32(orig), _f32(dir, orig.device)
+    near = torch.empty(o.shape[0], device=o.device)
+    far = torch.empty(o.shape[0], device=o.device)
+    with torch.cuda.device(o.device):
+        ctx.check(ctx.lib.nm_near_far_mesh(ctx.h, int(actor), _p(o), _p(d), o.shape[0], float(geo_threshold),
+                                           _p(near), _p(far), ctx.stream()))
+    return near, far
+
+
 def ray_to_samples(ray_batch, samples_per_ray, lindisp=False, perturb=0., device='cuda', append_t=None, t_rand=None):
     """utils/ray_utils.py:96-135 -> (pts [R,S,3], dirs [R,S,3], z_vals [R,S])."""
     if append_t is not None:
