@@ -98,6 +98,20 @@ typedef struct {
  *   the frame drivers accept any mix of kinds over their coarse, fine and human slots. */
 int nm_net_pack_noview(nm_ctx* ctx, int slot, const nm_nerf_noview_desc* desc, void* stream);
 
+/* Packs a NeRF-T net (the reference's --ablate_nerft background nets, train.py:254-256: the position input is
+ * (x, y, z, t), models/vanilla.py:60-79 with input_dims = 4) into `slot`: an nm_nerf_desc whose pts_linears.0 is
+ * [256,84] and .5 [256,340] (columns in the reference's order [x, y, z, t, sin(f_0 xyzt), cos(f_0 xyzt), ...]).  Only
+ * the posenc position mapping is accepted (the reference's rotate mapping asserts a 3-D input, models/vanilla.py:84).
+ * For a NeRF-T slot:
+ *   nm_mlp_forward / nm_mlp_forward_train read pts as [n,4] = (x, y, z, t), exactly the reference's input_pts; the stash
+ *   and nm_mlp_backward are those of a view-dependent net;
+ *   nm_encode_f16 with which = 0 reads x as [n,4] and writes [n][96]: the 84 channels in the reference's column order,
+ *   1.0 at channel 84, zeros to 95 (g^T @ plane = pts_linears.0's weight gradient, bias gradient in column 84);
+ *   nm_render_vanilla_t renders a frame at one time;
+ *   nm_mlp_forward_rays, nm_pe_backward with which = 0 (no input gradient) and the drivers without a time argument
+ *   (nm_render_vanilla, nm_render_smpl_nerf, nm_render_hybrid) return NM_ERR_UNSUPPORTED. */
+int nm_net_pack_nerft(nm_ctx* ctx, int slot, const nm_nerf_desc* desc, void* stream);
+
 /* Joiner.forward(input_pts, input_views) (models/vanilla.py:162-166) = Embedder.forward (:82-92)
  * on both inputs + NeRF.forward (:120-152).  pts, views: [n,3]; raw: [n,4].
  * If views_per_ray != 0, `views` is [n/views_per_ray, 3] and row i serves samples
@@ -322,6 +336,12 @@ typedef struct {
 int nm_render_vanilla(nm_ctx* ctx, int coarse_slot, int fine_slot /* -1 = none */,
                       const nm_camera* cam, const nm_render_opts* opt, int64_t pix0, int64_t n,
                       const int32_t* pixels, float* rgb, float* depth, int32_t host_out, void* stream);
+/* render_vanilla(..., ablate_nerft=True) (utils/render_utils.py:134-148) of NeRF-T coarse (and fine) nets: every sample
+ * carries the time `frame_time` (the reference's float32 frame_id / total_frames).  Arguments otherwise as
+ * nm_render_vanilla, whose chunk loop it shares. */
+int nm_render_vanilla_t(nm_ctx* ctx, int coarse_slot, int fine_slot /* -1 = none */,
+                        const nm_camera* cam, const nm_render_opts* opt, float frame_time, int64_t pix0, int64_t n,
+                        const int32_t* pixels, float* rgb, float* depth, int32_t host_out, void* stream);
 int nm_render_smpl_nerf(nm_ctx* ctx, int human_slot, int actor, const nm_camera* cam,
                         const nm_render_opts* opt, int64_t pix0, int64_t n, const int32_t* pixels, float* rgb,
                         float* depth, float* acc, int32_t host_out, void* stream);

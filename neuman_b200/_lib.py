@@ -62,6 +62,7 @@ SIGNATURES = {
     "nm_launch_count": (_I64, [_P]),
     "nm_net_pack": (C.c_int, [_P, C.c_int, C.POINTER(NmNerfDesc), _P]),
     "nm_net_pack_noview": (C.c_int, [_P, C.c_int, C.POINTER(NmNerfNoviewDesc), _P]),
+    "nm_net_pack_nerft": (C.c_int, [_P, C.c_int, C.POINTER(NmNerfDesc), _P]),
     "nm_mlp_forward": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _I64, _I32, _P, _P]),
     "nm_mlp_forward_train": (C.c_int, [_P, C.c_int, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
     "nm_encode_f16": (C.c_int, [_P, C.c_int, _I32, _P, _I64, _I64, _P, _P]),
@@ -92,6 +93,8 @@ SIGNATURES = {
     "nm_smpl_scene_backward": (C.c_int, [_P, C.POINTER(NmSmplModel), _P, _P, _P, _P, _F, _P, _P, _P, _P, _P, _P]),
     "nm_render_vanilla": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(NmCamera), C.POINTER(NmRenderOpts), _I64, _I64, _P,
                                     _P, _P, _I32, _P]),
+    "nm_render_vanilla_t": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(NmCamera), C.POINTER(NmRenderOpts), _F, _I64, _I64,
+                                      _P, _P, _P, _I32, _P]),
     "nm_render_smpl_nerf": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(NmCamera), C.POINTER(NmRenderOpts), _I64, _I64, _P,
                                       _P, _P, _P, _I32, _P]),
     "nm_render_hybrid": (C.c_int, [_P, C.c_int, C.c_int, _I32, C.POINTER(_I32), C.POINTER(_I32), _I32,

@@ -84,7 +84,7 @@ class _JoinerMLP(torch.autograd.Function):
         n = pts.shape[0]
         dev = pts.device
         h = dict(device=dev, dtype=torch.float16)
-        viewless = ops.is_viewless(joiner)
+        viewless = ops.is_viewless(joiner)                             # (NeRF-T nets: view-dependent, pts [n,4])
         sx = torch.empty(8, n, 256, **h)
         sf = sv = None                                                 # view-independent nets: no feature / views layer
         if not viewless:
@@ -159,12 +159,13 @@ def _input_grad(joiner, P, x, which, terms, inv):
 
 
 def _encodings(joiner, pts, views):
-    """The fp16 encodings as the forward kernel multiplied them ([n,64] / [n,32], with their constant-1 channel); a
-    view-independent net has no direction encoding (None)."""
+    """The fp16 encodings as the forward kernel multiplied them ([n,64] / [n,32], with their constant-1 channel right
+    after the encoding; a NeRF-T net's position plane is [n,96] in the reference's column order); a view-independent net
+    has no direction encoding (None)."""
     ctx = _ctx_for(pts)
     slot = ops.net_slot(joiner, ctx)
     n = pts.shape[0]
-    spe = torch.empty(n, 64, device=pts.device, dtype=torch.float16)
+    spe = torch.empty(n, 96 if ops.is_nerft(joiner) else 64, device=pts.device, dtype=torch.float16)
     ctx.check(ctx.lib.nm_encode_f16(ctx.h, slot, 0, _p(pts), 0, n, _p(spe), ctx.stream()))
     if ops.is_viewless(joiner):
         return spe, None
@@ -182,7 +183,7 @@ def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
     sx, sf, sv, _ = stash
     spe, sdpe = _encodings(joiner, pts, views)
     ctx = _ctx_for(g)
-    n_pe = joiner.pos_pe.out_dim                                          # 63: the 1.0 channel sits right after
+    n_pe = joiner.pos_pe.out_dim                                          # 63 (NeRF-T: 84): the 1.0 channel sits right after
     grads = {}
     g8 = torch.zeros(g.shape[0], 8, device=g.device, dtype=torch.float16)
     g8[:, :4] = g * (1.0 / inv)
@@ -197,7 +198,7 @@ def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
         grads['rgb_linear.bias'] = g[:, :3].sum(0)
         grads['alpha_linear.weight'] = _mm32(g8t, sx[7])[3:4] * inv
         grads['alpha_linear.bias'] = g[:, 3].sum().reshape(1)
-    w0 = _mm32(g_pre[0].t(), spe) * inv                                   # [256,64]: column 63 = bias gradient (1.0 channel)
+    w0 = _mm32(g_pre[0].t(), spe) * inv                                   # [256,64]: column 63 (84) = bias gradient (1.0 channel)
     dw, db = _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, g.shape[0])
     dw, db = dw * inv, db * inv
     if sdpe is not None:
@@ -245,9 +246,14 @@ def _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, n):
 
 def joiner_forward(joiner, input_pts, input_views=None):
     """Joiner.forward (models/vanilla.py:162-166) with gradients to the network parameters and, when they require
-    grad, to input_pts / input_views.  A view-independent net ignores input_views (may be None); its gradient is None."""
+    grad, to input_pts / input_views.  A view-independent net ignores input_views (may be None); its gradient is None.
+    A NeRF-T net takes input_pts [...,4] = (x, y, z, t); its inputs get no gradient (nothing in the reference
+    differentiates through them)."""
+    nerft = ops.is_nerft(joiner)
+    if nerft and (input_pts.requires_grad or (input_views is not None and input_views.requires_grad)):
+        raise NotImplementedError("input gradients of NeRF-T nets (ablate_nerft) are not built")
     shape = input_pts.shape[:-1]
-    pts = input_pts.float().contiguous().reshape(-1, 3)          # autograd-tracked views of the inputs
+    pts = input_pts.float().contiguous().reshape(-1, 4 if nerft else 3)   # autograd-tracked views of the inputs
     views = None
     if not ops.is_viewless(joiner):
         views = input_views.to(pts.device).float().contiguous().reshape(-1, 3)

@@ -180,18 +180,27 @@ static void pe_cycles_table(int kind, float fmin, float fmax, int nf, std::vecto
     }
 }
 
-// Packs a validated description of either kind into `slot`.  For a view-independent net (kind NM_NET_NOVIEW) `d` carries
+// Packs a validated description of any kind into `slot`.  For a view-independent net (kind NM_NET_NOVIEW) `d` carries
 // the trunk and the position encoding, its head pointers are null and its direction-encoding fields a fixed placeholder;
-// out_w / out_b are output_linear's weight and bias.
+// out_w / out_b are output_linear's weight and bias.  A NeRF-T net (NM_NET_NERFT) has pts_linears.0 [256,84] and .5
+// [256,340]; the fp32 layout is sized for them, so a slot that changes between NeRF-T and the other kinds is reallocated.
 static int net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, int kind, const float* out_w, const float* out_b,
                     cudaStream_t st) {
   NmNet& n = ctx->nets[slot];
+  const int KP = kind == NM_NET_NERFT ? NM_POS_PE_T : NM_POS_PE;
+  if (n.f32 && n.f32_pos_k != KP) {
+    NM_CHECK_CUDA(ctx, cudaDeviceSynchronize());      // work already queued may still read the old weights
+    NM_CHECK_CUDA(ctx, cudaFree(n.f32));
+    n.f32 = nullptr;
+    n.packed = false;
+    n.pe_valid = false;                               // the encoding tables live in the freed layout
+  }
   if (!n.f32) {
     // layout (floats)
     size_t off = 0;
     auto take = [&](size_t cnt) { size_t o = off; off += (cnt + 63) & ~size_t(63); return o; };
     for (int l = 0; l < 8; ++l) {
-      int K = (l == 0) ? NM_POS_PE : (l == 5 ? NM_POS_PE + NM_WIDTH : NM_WIDTH);
+      int K = (l == 0) ? KP : (l == 5 ? KP + NM_WIDTH : NM_WIDTH);
       n.o_pts_w[l] = take((size_t)K * NM_WIDTH);
       n.o_pts_b[l] = take(NM_WIDTH);
     }
@@ -203,6 +212,7 @@ static int net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, int kind, cons
     n.o_pos_cyc = take(192); n.o_dir_cyc = take(192);
     n.o_out_w = take((size_t)NM_WIDTH * 4); n.o_out_b = take(4);
     n.f32_floats = off;
+    n.f32_pos_k = KP;
     NM_CHECK_CUDA(ctx, cudaMalloc(&n.f32, off * sizeof(float)));
   }
   n.desc = *d;
@@ -217,11 +227,11 @@ static int net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, int kind, cons
     return cudaMemcpyAsync(n.f32 + dst_off, src, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st);
   };
   for (int l = 0; l < 8; ++l) {
-    int K = (l == 0) ? NM_POS_PE : (l == 5 ? NM_POS_PE + NM_WIDTH : NM_WIDTH);
+    int K = (l == 0) ? KP : (l == 5 ? KP + NM_WIDTH : NM_WIDTH);
     tr(d->pts_w[l], n.o_pts_w[l], NM_WIDTH, K);
     NM_CHECK_CUDA(ctx, cp(d->pts_b[l], n.o_pts_b[l], NM_WIDTH));
   }
-  if (kind == NM_NET_VIEW) {
+  if (kind != NM_NET_NOVIEW) {
     tr(d->feature_w, n.o_feat_w, NM_WIDTH, NM_WIDTH);
     NM_CHECK_CUDA(ctx, cp(d->feature_b, n.o_feat_b, NM_WIDTH));
     tr(d->alpha_w, n.o_alpha_w, 1, NM_WIDTH);
@@ -268,17 +278,35 @@ static int net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, int kind, cons
   return NM_OK;
 }
 
+static int check_view_desc(nm_ctx* ctx, const nm_nerf_desc* d, const char* who) {
+  for (int l = 0; l < 8; ++l)
+    if (!d->pts_w[l] || !d->pts_b[l]) NM_FAIL(ctx, NM_ERR_INVALID, std::string(who) + ": null pts_linears");
+  if (!d->feature_w || !d->feature_b || !d->alpha_w || !d->alpha_b || !d->views_w || !d->views_b || !d->rgb_w ||
+      !d->rgb_b)
+    NM_FAIL(ctx, NM_ERR_INVALID, std::string(who) + ": null head weights (use_viewdirs=True nets only)");
+  return NM_OK;
+}
+
 extern "C" int nm_net_pack(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* stream) {
   NM_ENTER(ctx);
   if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !d) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: bad slot/desc");
   if (d->pos_n_freqs != 10 || d->dir_n_freqs != 4)
     NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_net_pack: only pos_N_freqs=10 / dir_N_freqs=4 (63/27-d encodings) is built");
-  for (int l = 0; l < 8; ++l)
-    if (!d->pts_w[l] || !d->pts_b[l]) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: null pts_linears");
-  if (!d->feature_w || !d->feature_b || !d->alpha_w || !d->alpha_b || !d->views_w || !d->views_b || !d->rgb_w ||
-      !d->rgb_b)
-    NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack: null head weights (use_viewdirs=True nets only)");
+  const int rc = check_view_desc(ctx, d, __func__);
+  if (rc != NM_OK) return rc;
   return net_pack(ctx, slot, d, NM_NET_VIEW, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int nm_net_pack_nerft(nm_ctx* ctx, int slot, const nm_nerf_desc* d, void* stream) {
+  NM_ENTER(ctx);
+  if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !d) NM_FAIL(ctx, NM_ERR_INVALID, "nm_net_pack_nerft: bad slot/desc");
+  if (d->pos_n_freqs != 10 || d->dir_n_freqs != 4)
+    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_net_pack_nerft: only pos_N_freqs=10 / dir_N_freqs=4 (84/27-d encodings) is built");
+  if (d->pos_pe_kind != NM_PE_POSENC)      // the reference's rotate mapping asserts a 3-D input (models/vanilla.py:84)
+    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_net_pack_nerft: the position encoding of a NeRF-T net must be posenc");
+  const int rc = check_view_desc(ctx, d, __func__);
+  if (rc != NM_OK) return rc;
+  return net_pack(ctx, slot, d, NM_NET_NERFT, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int nm_net_pack_noview(nm_ctx* ctx, int slot, const nm_nerf_noview_desc* d, void* stream) {
@@ -299,7 +327,7 @@ extern "C" int nm_net_pack_noview(nm_ctx* ctx, int slot, const nm_nerf_noview_de
 }
 
 static int mlp_dispatch(nm_ctx* ctx, int slot, int mode, const float* pts, const float* views, const float* origins,
-                        const float* dirs, const float* z, int64_t n, int32_t group, float* raw, void* stream,
+                        const float* dirs, const float* z, int64_t n, int32_t group, float t, float* raw, void* stream,
                         const NmTrainStash* stash = nullptr) {
   if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !ctx->nets[slot].packed)
     NM_FAIL(ctx, NM_ERR_STATE, "nm_mlp_forward: net slot not packed");
@@ -321,8 +349,8 @@ static int mlp_dispatch(nm_ctx* ctx, int slot, int mode, const float* pts, const
     e1 = ctx->prof_events[ctx->prof_used + 1];
     NM_CHECK_CUDA(ctx, cudaEventRecord(e0, st));
   }
-  int rc = mode == NM_MLP_SIMT_F32 ? nm_simt_forward(ctx, net, pts, views, origins, dirs, z, n, group, raw, st)
-                                   : nm_tc_forward(ctx, net, pts, views, origins, dirs, z, n, group, raw, st, stash);
+  int rc = mode == NM_MLP_SIMT_F32 ? nm_simt_forward(ctx, net, pts, views, origins, dirs, z, n, group, t, raw, st)
+                                   : nm_tc_forward(ctx, net, pts, views, origins, dirs, z, n, group, t, raw, st, stash);
   if (ctx->profile && rc == NM_OK) {
     NM_CHECK_CUDA(ctx, cudaEventRecord(e1, st));
     ctx->prof_used += 2;
@@ -338,6 +366,9 @@ static bool views_ok(const nm_ctx* ctx, int slot, const void* views) {
 static bool is_noview(const nm_ctx* ctx, int slot) {
   return slot >= 0 && slot < NM_MAX_NET_SLOTS && ctx->nets[slot].kind == NM_NET_NOVIEW;
 }
+static bool is_nerft(const nm_ctx* ctx, int slot) {
+  return slot >= 0 && slot < NM_MAX_NET_SLOTS && ctx->nets[slot].packed && ctx->nets[slot].kind == NM_NET_NERFT;
+}
 
 extern "C" int nm_mlp_forward(nm_ctx* ctx, int slot, int mode, const float* pts, const float* views, int64_t n,
                               int32_t views_per_ray, float* raw, void* stream) {
@@ -345,7 +376,7 @@ extern "C" int nm_mlp_forward(nm_ctx* ctx, int slot, int mode, const float* pts,
   if (!pts || !views_ok(ctx, slot, views) || views_per_ray < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward: null pts/views");
   if (views_per_ray > 0 && n % views_per_ray != 0)
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward: n is not a multiple of views_per_ray");
-  return mlp_dispatch(ctx, slot, mode, pts, views, nullptr, nullptr, nullptr, n, views_per_ray, raw, stream);
+  return mlp_dispatch(ctx, slot, mode, pts, views, nullptr, nullptr, nullptr, n, views_per_ray, 0.f, raw, stream);
 }
 
 extern "C" int nm_mlp_forward_train(nm_ctx* ctx, int slot, const float* pts, const float* views, int64_t n,
@@ -360,7 +391,7 @@ extern "C" int nm_mlp_forward_train(nm_ctx* ctx, int slot, const float* pts, con
   if (views_per_ray > 0 && n % views_per_ray != 0)
     NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_train: n is not a multiple of views_per_ray");
   NmTrainStash sh{(__half*)stash_x, (__half*)stash_f, (__half*)stash_v, (uint32_t*)stash_m};
-  return mlp_dispatch(ctx, slot, NM_MLP_TC_F16, pts, views, nullptr, nullptr, nullptr, n, views_per_ray, raw, stream, &sh);
+  return mlp_dispatch(ctx, slot, NM_MLP_TC_F16, pts, views, nullptr, nullptr, nullptr, n, views_per_ray, 0.f, raw, stream, &sh);
 }
 
 extern "C" int nm_mlp_backward(nm_ctx* ctx, int slot, const float* d_raw, const float* loss_scale, int64_t n,
@@ -397,6 +428,8 @@ extern "C" int nm_pe_backward(nm_ctx* ctx, int slot, int32_t which, const float*
     NM_FAIL(ctx, NM_ERR_STATE, "nm_pe_backward: net slot not packed");
   if ((which != 0 && which != 1) || n < 0 || group < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_pe_backward: bad argument");
   if (which == 1 && is_noview(ctx, slot)) NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_pe_backward: view-independent net has no direction encoding");
+  if (which == 0 && is_nerft(ctx, slot))           // nothing in the reference differentiates through a NeRF-T net's input
+    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_pe_backward: no position-input gradient for NeRF-T nets");
   const NmNet& net = ctx->nets[slot];
   const int width = 3 + 6 * (which == 0 ? net.desc.pos_n_freqs : net.desc.dir_n_freqs);
   if (ld < width) NM_FAIL(ctx, NM_ERR_INVALID, "nm_pe_backward: ld smaller than the encoding width");
@@ -421,9 +454,15 @@ extern "C" int nm_dw_gemm(nm_ctx* ctx, const void* g_pre, const void* g_f, const
                          (const __half*)stash_f, n, out, bias_out, (cudaStream_t)stream);
 }
 
+int nm_impl_mlp_forward_rays(nm_ctx* ctx, int slot, int mode, const float* origins, const float* dirs, const float* z,
+                             int64_t R, int32_t S, float t, float* raw, cudaStream_t st) {
+  if (!origins || !dirs || !z || S <= 0 || R < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_rays: bad argument");
+  return mlp_dispatch(ctx, slot, mode, nullptr, nullptr, origins, dirs, z, R * (int64_t)S, S, t, raw, st);
+}
+
 extern "C" int nm_mlp_forward_rays(nm_ctx* ctx, int slot, int mode, const float* origins, const float* dirs,
                                    const float* z, int64_t R, int32_t S, float* raw, void* stream) {
   NM_ENTER(ctx);
-  if (!origins || !dirs || !z || S <= 0 || R < 0) NM_FAIL(ctx, NM_ERR_INVALID, "nm_mlp_forward_rays: bad argument");
-  return mlp_dispatch(ctx, slot, mode, nullptr, nullptr, origins, dirs, z, R * (int64_t)S, S, raw, stream);
+  if (is_nerft(ctx, slot)) NM_FAIL(ctx, NM_ERR_UNSUPPORTED, "nm_mlp_forward_rays: a NeRF-T net needs the time (nm_render_vanilla_t)");
+  return nm_impl_mlp_forward_rays(ctx, slot, mode, origins, dirs, z, R, S, 0.f, raw, (cudaStream_t)stream);
 }

@@ -64,35 +64,48 @@ __device__ __forceinline__ void zero_acc(float (&acc)[8][NJ]) {
 }
 
 // kView: use_viewdirs=True (alpha, feature, views and rgb heads); otherwise output_linear on layer 7 (:145-146) and no
-// direction input
-template <bool kView>
+// direction input.  kTime: a NeRF-T net (view-dependent, position input (x, y, z, t)): its 84-wide position encoding is
+// built in the reference's column order, so pts_linears.0 / .5 are used as given.
+template <bool kView, bool kTime = false>
 __device__ __forceinline__ void mlp_simt_body(const SimtParams& P, const NmMlpInput& in, float* __restrict__ raw) {
+  constexpr int PE_LD = kTime ? 96 : 64;
   extern __shared__ float sm[];
   float* hA = sm;                    // [64][256]
   float* hB = hA + TM * 256;         // [64][256]
-  float* pe = hB + TM * 256;         // [64][64]  (63 used)
-  float* vpe = pe + TM * 64;         // [64][32]  (27 used)
+  float* pe = hB + TM * 256;         // [64][PE_LD]  (63 / 84 used)
+  float* vpe = pe + TM * PE_LD;      // [64][32]  (27 used)
   float* s_alpha = vpe + TM * 32;    // [64]
   const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
   const long long base = (long long)blockIdx.x * TM;
 
   // ---- positional encodings ----
-  const int npos = 3 * P.pos_pe.n_freqs, ndir = kView ? 3 * P.dir_pe.n_freqs : 0;
+  const int npos = (kTime ? 4 : 3) * P.pos_pe.n_freqs, ndir = kView ? 3 * P.dir_pe.n_freqs : 0;
   for (int t = tid; t < TM * (npos + ndir + 2); t += NT) {
     int s = t / (npos + ndir + 2), q = t - s * (npos + ndir + 2);
     long long i = base + s;
-    float p[3] = {0, 0, 0}, v[3] = {0, 0, 0};
-    if (i < in.n) nm_fetch_sample(in, i, p, v);
-    if (q < npos) {
+    float p[3] = {0, 0, 0}, v[3] = {0, 0, 0}, tm = 0.f;
+    if (i < in.n) {
+      nm_fetch_sample<kTime ? 4 : 3>(in, i, p, v);
+      if (kTime) tm = nm_fetch_time(in, i);
+    }
+    if (kTime && q < npos) {
+      // Embedder.forward with input_dims = 4 (:69-75): sin(x f_k) at column 4 + 8k + d, cos at 8 + 8k + d (d = 3: time)
+      const int k = q >> 2, d = q & 3;
+      float sn, cs;
+      sincosf((d < 3 ? p[d] : tm) * P.pos_pe.table[k], &sn, &cs);
+      pe[s * PE_LD + 4 + 8 * k + d] = sn; pe[s * PE_LD + 8 + 8 * k + d] = cs;
+    } else if (q < npos) {
       float sn, cs; int ci, cj;
       nm_pe_pair(P.pos_pe, p, q, sn, cs, ci, cj);
-      pe[s * 64 + ci] = sn; pe[s * 64 + cj] = cs;
+      pe[s * PE_LD + ci] = sn; pe[s * PE_LD + cj] = cs;
     } else if (q < npos + ndir) {
       float sn, cs; int ci, cj;
       nm_pe_pair(P.dir_pe, v, q - npos, sn, cs, ci, cj);
       vpe[s * 32 + ci] = sn; vpe[s * 32 + cj] = cs;
     } else if (q == npos + ndir) {
-      pe[s * 64 + 0] = p[0]; pe[s * 64 + 1] = p[1]; pe[s * 64 + 2] = p[2]; pe[s * 64 + 63] = 0.f;
+      pe[s * PE_LD + 0] = p[0]; pe[s * PE_LD + 1] = p[1]; pe[s * PE_LD + 2] = p[2];
+      if (kTime) pe[s * PE_LD + 3] = tm;
+      else pe[s * PE_LD + 63] = 0.f;
     } else if (kView) {
       vpe[s * 32 + 0] = v[0]; vpe[s * 32 + 1] = v[1]; vpe[s * 32 + 2] = v[2];
 #pragma unroll
@@ -101,21 +114,21 @@ __device__ __forceinline__ void mlp_simt_body(const SimtParams& P, const NmMlpIn
   }
   __syncthreads();
 
-  const int KP = 3 + 2 * npos;   // 63
+  const int KP = kTime ? NM_POS_PE_T : 3 + 2 * npos;   // 63 / 84
   const int KV = 3 + 2 * ndir;   // 27
   float acc[8][8];
   float* cur = hA;
   float* nxt = hB;
   // layer 0
   zero_acc(acc);
-  gemm_acc<8>(acc, pe, 64, KP, P.w[0], 256, tx, ty);
+  gemm_acc<8>(acc, pe, PE_LD, KP, P.w[0], 256, tx, ty);
   store_out<8>(acc, P.b[0], true, cur, 256, tx, ty);
   __syncthreads();
   for (int l = 1; l < 8; ++l) {
     zero_acc(acc);
     const float* W = P.w[l];
     if (l == 5) {                                   // cat([input_pts, h]) (models/vanilla.py:131)
-      gemm_acc<8>(acc, pe, 64, KP, W, 256, tx, ty);
+      gemm_acc<8>(acc, pe, PE_LD, KP, W, 256, tx, ty);
       W += (size_t)KP * 256;
     }
     gemm_acc<8>(acc, cur, 256, 256, W, 256, tx, ty);
@@ -178,9 +191,12 @@ __global__ void __launch_bounds__(NT, 1) k_mlp_simt(SimtParams P, NmMlpInput in,
 __global__ void __launch_bounds__(NT, 1) k_mlp_simt_noview(SimtParams P, NmMlpInput in, float* __restrict__ raw) {
   mlp_simt_body<false>(P, in, raw);
 }
+__global__ void __launch_bounds__(NT, 1) k_mlp_simt_nerft(SimtParams P, NmMlpInput in, float* __restrict__ raw) {
+  mlp_simt_body<true, true>(P, in, raw);
+}
 
 int nm_simt_forward(nm_ctx* ctx, const NmNet& net, const float* pts, const float* views, const float* origins,
-                    const float* dirs, const float* z, int64_t n, int32_t group, float* raw, cudaStream_t st) {
+                    const float* dirs, const float* z, int64_t n, int32_t group, float t, float* raw, cudaStream_t st) {
   SimtParams P;
   for (int l = 0; l < 8; ++l) { P.w[l] = net.f32 + net.o_pts_w[l]; P.b[l] = net.f32 + net.o_pts_b[l]; }
   P.feat_w = net.f32 + net.o_feat_w; P.feat_b = net.f32 + net.o_feat_b;
@@ -190,10 +206,14 @@ int nm_simt_forward(nm_ctx* ctx, const NmNet& net, const float* pts, const float
   P.out_w = net.f32 + net.o_out_w; P.out_b = net.f32 + net.o_out_b;
   P.pos_pe = {net.desc.pos_pe_kind, net.desc.pos_n_freqs, net.f32 + net.o_pos_bv};
   P.dir_pe = {net.desc.dir_pe_kind, net.desc.dir_n_freqs, net.f32 + net.o_dir_bv};
-  NmMlpInput in{pts, views, origins, dirs, z, (long long)n, group};
+  NmMlpInput in{pts, views, origins, dirs, z, (long long)n, group, t};
   size_t smem = (size_t)(2 * TM * 256 + TM * 64 + TM * 32 + TM) * sizeof(float);
   unsigned blocks = (unsigned)((n + TM - 1) / TM);
-  if (net.kind == NM_NET_VIEW) {
+  if (net.kind == NM_NET_NERFT) {
+    smem += (size_t)TM * (96 - 64) * sizeof(float);
+    NM_SET_SMEM_ONCE(ctx, (k_mlp_simt_nerft), (int)smem);
+    k_mlp_simt_nerft<<<blocks, NT, smem, st>>>(P, in, raw);
+  } else if (net.kind == NM_NET_VIEW) {
     NM_SET_SMEM_ONCE(ctx, (k_mlp_simt), (int)smem);
     k_mlp_simt<<<blocks, NT, smem, st>>>(P, in, raw);
   } else {

@@ -26,7 +26,7 @@
 // Plan: which slabs a step consumes, where they live in the packed image.
 // ---------------------------------------------------------------------------------------------
 struct TcPlan {
-  uint32_t slab_off[TC_STEPS][5];   // byte offset inside the image
+  uint32_t slab_off[TC_STEPS][6];   // byte offset inside the image
   uint32_t slab_bytes[TC_STEPS];    // bytes per slab of this step
   uint32_t image_bytes;             // size of the image
 };
@@ -40,19 +40,28 @@ struct TcPlan {
 // `v` selects the net kind: true = view-dependent (steps 0-10 above), false = view-independent (use_viewdirs=False,
 // models/vanilla.py:145-146): steps 0-7 as above, then step 8 = output_linear (N = 16, 4 used, K = 256 over the layer-7
 // activation block, :146); no alpha, feature, views or rgb step, no direction encoding.
+// `t` selects a NeRF-T net (view-dependent, position input (x, y, z, t), train.py:254-256): the 21 time channels t, sin(f_k t),
+// cos(f_k t) sit in channels 32..52 of the direction-encoding block (the views step reads only its channels 0..31), and steps
+// 0 and 5 get one more k-block, a "time slab" (last k-block of the step) consumed by two K = 16 MMAs on K slices 2..3 of that
+// block, like the bias slab.
 __host__ __device__ constexpr int tc_steps(bool v) { return v ? TC_STEPS : 9; }
-__host__ __device__ constexpr int step_nkb(int s, bool v = true) { return s == 0 ? 1 : (s == 10 ? 2 : (!v && s == 8 ? 4 : 5)); }
+__host__ __device__ constexpr int step_nkb(int s, bool v = true, bool t = false) {
+  return s == 0 ? (t ? 2 : 1) : (s == 10 ? 2 : (!v && s == 8 ? 4 : (t && s == 5 ? 6 : 5)));
+}
 __host__ __device__ constexpr bool kb_is_bias(int s, int kb, bool v = true) {
   return kb == 4 && s != 5 && s != 9 && s >= 1 && (v ? s <= 8 : s <= 7);
 }
+__host__ __device__ constexpr bool kb_is_time(int s, int kb, bool t) { return t && ((s == 0 && kb == 1) || (s == 5 && kb == 5)); }
 __host__ __device__ constexpr int step_N(int s, bool v = true) { return s <= 7 || (v && s == 8) ? 256 : (v && s == 9 ? 128 : 16); }
 // k-block kb of step s reads the position encoding / the direction encoding (else activation block `act_kb`)
-__host__ __device__ constexpr bool kb_is_pos(int s, int kb, bool v = true) { return (s == 0) || (s == 5 && kb == 0) || kb_is_bias(s, kb, v); }
+__host__ __device__ constexpr bool kb_is_pos(int s, int kb, bool v = true, bool t = false) {
+  return (s == 0 && (!t || kb == 0)) || (s == 5 && kb == 0) || kb_is_bias(s, kb, v);
+}
 __host__ __device__ constexpr bool kb_is_dir(int s, int kb, bool v = true) { return v && s == 9 && kb == 4; }
 __host__ __device__ constexpr int kb_act_index(int s, int kb) { return s == 5 ? kb - 1 : kb; }
-__host__ __device__ constexpr int tc_slabs_per_tile(bool v = true) {
+__host__ __device__ constexpr int tc_slabs_per_tile(bool v = true, bool t = false) {
   int n = 0;
-  for (int s = 0; s < tc_steps(v); ++s) n += step_nkb(s, v);
+  for (int s = 0; s < tc_steps(v); ++s) n += step_nkb(s, v, t);
   return n;
 }
 
@@ -153,6 +162,22 @@ __device__ __forceinline__ void encode_f16(const NmPeSpec& pe, const float x[3],
   for (int i = 0; i < 32; ++i) out[i] = pack_f16x2(ch[2 * i], ch[2 * i + 1], false);
 }
 
+// Encodes the time t of a NeRF-T net into channels 32..52 of a direction-encoding row (out[16..26]): channel 32 = t,
+// 33 + 2k = sin(f_k t), 34 + 2k = cos(f_k t), with the position encoding's frequencies (posenc table, as encode_f16).
+__device__ __forceinline__ void encode_time_f16(const NmPeSpec& pe, float t, uint32_t (&out)[32]) {
+  float ch[22];
+  ch[0] = t; ch[21] = 0.f;
+#pragma unroll
+  for (int k = 0; k < 10; ++k) {
+    const float fh = __ldg(pe.table + 2 * k), fl = __ldg(pe.table + 2 * k + 1);
+    const float pr = t * fh;
+    const float low = fmaf(t, fl, fmaf(t, fh, -pr));
+    sincos_cycles((pr - rintf(pr)) + low, ch[1 + 2 * k], ch[2 + 2 * k]);
+  }
+#pragma unroll
+  for (int i = 0; i < 11; ++i) out[16 + i] = pack_f16x2(ch[2 * i], ch[2 * i + 1], false);
+}
+
 // write 8 * nchunks f16 of one 128-byte row of a K block with the 128B swizzle
 __device__ __forceinline__ void store_row_swizzled(uint8_t* blk, int row, const uint32_t* v, int nchunks) {
 #pragma unroll
@@ -229,10 +254,11 @@ __device__ __forceinline__ void quad_or(uint32_t (&w)[8]) {
 // ---------------------------------------------------------------------------------------------
 // The kernel body, shared by the view-dependent (kView) and view-independent nets: same tile loop, same ring, same steps 0-7
 // ---------------------------------------------------------------------------------------------
-template <bool kTrain, bool kView>
+template <bool kTrain, bool kView, bool kTime = false>
 __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
+  static_assert(!kTime || kView, "NeRF-T nets are view-dependent");
   using C = TcCfg;
-  constexpr int SLABS = tc_slabs_per_tile(kView);
+  constexpr int SLABS = tc_slabs_per_tile(kView, kTime);
   constexpr int STEPS = tc_steps(kView);
   constexpr int LAST = STEPS - 1;                       // the output step: rgb (N = 16) or output_linear (N = 16)
   extern __shared__ uint8_t smem_dyn[];
@@ -260,7 +286,7 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
     mbar_arrive_expect_tx(R.full(pq), bytes);
     bulk_g2s(R.slot(pq), P.wimg + P.plan.slab_off[ps][pkb], bytes, R.full(pq));
     ++pq;
-    if (++pkb == step_nkb(ps, kView)) { pkb = 0; if (++ps == STEPS) ps = 0; }
+    if (++pkb == step_nkb(ps, kView, kTime)) { pkb = 0; if (++ps == STEPS) ps = 0; }
   };
   if (threadIdx.x == 0) {
     R.init();
@@ -298,33 +324,41 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
       const uint32_t off = wg * TC_WG_ROWS + r;            // row0 + r - tile * 128
       const long long g = group > 0 ? g0 + (g0r + off) / (uint32_t)group : row0 + r;
       float p[3] = {0.f, 0.f, 0.f}, v[3] = {0.f, 0.f, 0.f};
-      if (row0 + r < P.in.n) nm_fetch_sample_at(P.in, row0 + r, g, p, v);
+      float t = 0.f;
+      if (row0 + r < P.in.n) {
+        nm_fetch_sample_at<kTime ? 4 : 3>(P.in, row0 + r, g, p, v);
+        if (kTime) t = nm_fetch_time(P.in, row0 + r);
+      }
       uint32_t e[32];
       if (wtid < 64) {
         encode_f16(P.pos_pe, p, e, 30);
         store_row_swizzled(wbuf + C::OFF_POS, r, e, 8);
       } else if (kView) {
         encode_f16(P.dir_pe, v, e, 12);
-        store_row_swizzled(wbuf + C::OFF_DIR, r, e, 4);
+        if (kTime) encode_time_f16(P.pos_pe, t, e);
+        store_row_swizzled(wbuf + C::OFF_DIR, r, e, kTime ? 8 : 4);
       }
       if (track && (kView || wtid < 64)) { track_range<false>(rng, e[0]); track_range<false>(rng, e[1]); }   // raw x, y, z (+ one sine)
+      if (kTime && track && wtid >= 64) track_range<false>(rng, e[16]);                                       // t, sin(f_0 t)
       fence_async_smem();
       wg_sync(wg);
     }
     float alpha[2] = {0.f, 0.f};
     for (int s = 0; s < STEPS; ++s) {
-      const int nkb = step_nkb(s, kView);
+      const int nkb = step_nkb(s, kView, kTime);
       wgmma_fence();
       for (int kb = 0; kb < nkb; ++kb) {
         const uint32_t qq = qbase + kb;
         R.wait_full(qq);
-        const uint32_t a_addr = kb_is_pos(s, kb, kView) ? wbase + C::OFF_POS
-                              : kb_is_dir(s, kb, kView) ? wbase + C::OFF_DIR
+        const bool time = kb_is_time(s, kb, kTime);
+        const uint32_t a_addr = kb_is_pos(s, kb, kView, kTime) ? wbase + C::OFF_POS
+                              : (kb_is_dir(s, kb, kView) || time) ? wbase + C::OFF_DIR
                                                  : wbase + kb_act_index(s, kb) * TC_KB_BYTES;
         // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
-        // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab)
+        // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab), a time
+        // slab two on K slices 2..3 (channels 32..63 of the direction block)
         const bool bias = kb_is_bias(s, kb, kView);
-        const int k0 = bias ? 3 : 0, k1 = kb_is_dir(s, kb, kView) ? 2 : 4;
+        const int k0 = bias ? 3 : (time ? 2 : 0), k1 = kb_is_dir(s, kb, kView) ? 2 : 4;
         const uint64_t a_desc = gmma_desc_k(a_addr), b_desc = gmma_desc_k(R.slot(qq));
         for (int k = k0; k < k1; ++k) {
           const uint32_t acc = (kb | (k - k0)) != 0;
@@ -415,6 +449,11 @@ template <bool kTrain>
 __global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc_noview(const __grid_constant__ TcParams P) {
   mlp_tc_body<kTrain, false>(P);
 }
+// NeRF-T nets (view-dependent, position input (x, y, z, t)): render (kTrain = false) and training forward
+template <bool kTrain>
+__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc_nerft(const __grid_constant__ TcParams P) {
+  mlp_tc_body<kTrain, true, true>(P);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Packing: fp32 nn.Linear weights -> fp16 slabs in the swizzled GMMA layout.
@@ -425,12 +464,38 @@ struct PackSrc {
   const float* out_t;                                                 // output_linear.weight as [256][4] (view-independent nets)
 };
 
-// weight of (step s, output n, k-block kb, kk in [0,64)) or 0 for padding; `view` = the net kind (step tables above)
-__device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int kb, int kk, bool view) {
+// Column of a NeRF-T net's 84-wide encoding (the reference's order [x, y, z, t, sin(f_0 xyzt), cos(f_0 xyzt), ...],
+// models/vanilla.py:69-75 with input_dims = 4) that feeds channel kk of the kernel's position block (kk < 63: x, y, z, then
+// sin / cos of x, y, z per frequency as encode_f16 lays them out) or of its time channels (time = true, kk in 32..52);
+// -1 for a channel no column feeds.
+__device__ __forceinline__ int nerft_col(int kk, bool time) {
+  if (time) {
+    if (kk == 32) return 3;
+    if (kk < 33 || kk > 52) return -1;
+    const int k = (kk - 33) >> 1;
+    return ((kk - 33) & 1) ? 11 + 8 * k : 7 + 8 * k;
+  }
+  if (kk < 3) return kk;
+  const int i = kk - 3, k = i / 6, r = i - 6 * k;
+  return r < 3 ? 4 + 8 * k + r : 8 + 8 * k + (r - 3);
+}
+
+// weight of (step s, output n, k-block kb, kk in [0,64)) or 0 for padding; `view`, `time` = the net kind (step tables above)
+__device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int kb, int kk, bool view, bool time) {
   if (!view && s == 8) return n < 4 ? S.out_t[(size_t)(kb * 64 + kk) * 4 + n] : 0.f;   // output_linear, N padded 4 -> 16
   if (kb_is_bias(s, kb, view)) {                 // bias slab of a K = 256 step: only the column of PE channel 63 is non-zero
     if (kk != 63) return 0.f;
     return s == 8 ? S.feat_b[n] : S.b[s][n];
+  }
+  if (time && (s == 0 || s == 5)) {              // pts_linears.0 [256,84] / .5 [256,340]: columns in the reference's order
+    const int ld = s == 0 ? NM_POS_PE_T : NM_POS_PE_T + 256;
+    const float* w = S.w[s] + (size_t)n * ld;
+    if (kb_is_time(s, kb, true)) {
+      const int c = nerft_col(kk, true);
+      return c < 0 ? 0.f : w[c];
+    }
+    if (kb == 0) return kk < NM_POS_PE ? w[nerft_col(kk, false)] : S.b[s][n];                 // kk == 63: bias
+    return w[NM_POS_PE_T + (kb - 1) * 64 + kk];
   }
   if (s == 0) return kk < NM_POS_PE ? S.w[0][(size_t)n * NM_POS_PE + kk] : S.b[0][n];           // kk == 63: bias
   if (s >= 1 && s <= 7 && s != 5) return S.w[s][(size_t)n * 256 + kb * 64 + kk];
@@ -449,7 +514,7 @@ __device__ __forceinline__ float src_weight(const PackSrc& S, int s, int n, int 
   return n < 3 ? S.rgb[(size_t)n * 128 + kb * 64 + kk] : 0.f;
 }
 
-__global__ void k_tc_pack(PackSrc S, TcPlan plan, bool view, __half* __restrict__ out) {
+__global__ void k_tc_pack(PackSrc S, TcPlan plan, bool view, bool time, __half* __restrict__ out) {
   // one thread per packed element of the image
   const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;      // half index inside the image
   if (e * 2 >= plan.image_bytes) return;
@@ -457,14 +522,14 @@ __global__ void k_tc_pack(PackSrc S, TcPlan plan, bool view, __half* __restrict_
   // locate (s, kb)
   int s = 0, kb = 0;
   for (int ss = 0; ss < tc_steps(view); ++ss)
-    for (int k = 0; k < step_nkb(ss, view); ++k)
+    for (int k = 0; k < step_nkb(ss, view, time); ++k)
       if (byte >= plan.slab_off[ss][k]) { s = ss; kb = k; }
   const uint32_t in_slab = byte - plan.slab_off[s][kb];
   const int n = in_slab >> 7;
   const int chunk_phys = (in_slab & 127) >> 4;
   const int chunk = chunk_phys ^ (n & 7);                               // undo the 128B swizzle
   const int kk = chunk * 8 + ((in_slab & 15) >> 1);
-  out[e] = __float2half_rn(src_weight(S, s, n, kb, kk, view));
+  out[e] = __float2half_rn(src_weight(S, s, n, kb, kk, view, time));
 }
 
 // the constant table of the epilogue (layout: TC_CONST_ALPHA / TC_CONST_OUT)
@@ -508,28 +573,64 @@ __global__ void k_encode_f16(NmPeSpec pe, int which, const float* __restrict__ x
   }
 }
 
+// The position encoding of a NeRF-T net as the forward kernel feeds it to the MMAs (the same fp16 values: encode_f16 /
+// encode_time_f16 arithmetic), laid out in the reference's column order [x, y, z, t, sin(f_0 xyzt), cos(f_0 xyzt), ...]
+// (84 channels), then 1.0 at channel 84 and zeros to 95: [n][96].  g^T @ plane gives pts_linears.0's weight gradient in
+// the reference's layout and its bias gradient as column 84, so the kernel's channel permutation stays in this file.
+__global__ void k_encode_f16_nerft(NmPeSpec pe, const float* __restrict__ x, long long group, long long n,
+                                   __half* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long xi = group > 0 ? i / group : i;
+  float ch[96];
+#pragma unroll
+  for (int c = 0; c < 96; ++c) ch[c] = 0.f;
+#pragma unroll
+  for (int d = 0; d < 4; ++d) ch[d] = x[4 * xi + d];
+#pragma unroll
+  for (int k = 0; k < 10; ++k) {
+    const float fh = __ldg(pe.table + 2 * k), fl = __ldg(pe.table + 2 * k + 1);
+#pragma unroll
+    for (int d = 0; d < 4; ++d) {
+      const float v = ch[d];
+      const float pr = v * fh;
+      const float low = fmaf(v, fl, fmaf(v, fh, -pr));
+      sincos_cycles((pr - rintf(pr)) + low, ch[4 + 8 * k + d], ch[8 + 8 * k + d]);
+    }
+  }
+  ch[NM_POS_PE_T] = 1.f;
+  uint4* dst = reinterpret_cast<uint4*>(out + (size_t)i * 96);
+#pragma unroll
+  for (int j = 0; j < 12; ++j)
+    dst[j] = make_uint4(pack_f16x2(ch[8 * j], ch[8 * j + 1], false), pack_f16x2(ch[8 * j + 2], ch[8 * j + 3], false),
+                        pack_f16x2(ch[8 * j + 4], ch[8 * j + 5], false), pack_f16x2(ch[8 * j + 6], ch[8 * j + 7], false));
+}
+
 int nm_tc_encode(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64_t group, int64_t n, __half* out, cudaStream_t st) {
   NmPeSpec pe = which == 0 ? NmPeSpec{net.desc.pos_pe_kind, net.desc.pos_n_freqs, net.f32 + net.o_pos_cyc}
                            : NmPeSpec{net.desc.dir_pe_kind, net.desc.dir_n_freqs, net.f32 + net.o_dir_cyc};
-  k_encode_f16<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(pe, which, x, group, n, out);
+  if (which == 0 && net.kind == NM_NET_NERFT)
+    k_encode_f16_nerft<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(pe, x, group, n, out);
+  else
+    k_encode_f16<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(pe, which, x, group, n, out);
   NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }
 
-static TcPlan make_plan(bool view) {
+static TcPlan make_plan(bool view, bool time) {
   TcPlan p{};
   uint32_t off = 0;
   for (int s = 0; s < tc_steps(view); ++s) {
     p.slab_bytes[s] = (uint32_t)step_N(s, view) * 128u;
-    for (int kb = 0; kb < step_nkb(s, view); ++kb) { p.slab_off[s][kb] = off; off += p.slab_bytes[s]; }
+    for (int kb = 0; kb < step_nkb(s, view, time); ++kb) { p.slab_off[s][kb] = off; off += p.slab_bytes[s]; }
   }
   p.image_bytes = off;
   return p;
 }
 
 int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
-  const bool view = net.kind == NM_NET_VIEW;
-  TcPlan plan = make_plan(view);
+  const bool view = net.kind != NM_NET_NOVIEW, time = net.kind == NM_NET_NERFT;
+  TcPlan plan = make_plan(view, time);
   const size_t halfs = plan.image_bytes / 2;
   if (!net.f16 || net.f16_halfs != halfs) {
     if (net.f16) { NM_CHECK_CUDA(ctx, cudaDeviceSynchronize()); NM_CHECK_CUDA(ctx, cudaFree(net.f16)); net.f16 = nullptr; }
@@ -544,7 +645,7 @@ int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   for (int l = 0; l < 8; ++l) S.b[l] = d.pts_b[l];
   S.feat_b = d.feature_b; S.views_b = d.views_b;
   S.out_t = net.f32 + net.o_out_w;
-  k_tc_pack<<<(unsigned)((halfs + 255) / 256), 256, 0, st>>>(S, plan, view, net.f16);
+  k_tc_pack<<<(unsigned)((halfs + 255) / 256), 256, 0, st>>>(S, plan, view, time, net.f16);
   NM_CHECK_LAUNCH(ctx);
   if (view) k_tc_consts<<<1, 256, 0, st>>>(d.rgb_b, d.alpha_w, d.alpha_b, net.tc_bias);
   else k_tc_consts_noview<<<1, 256, 0, st>>>(net.f32 + net.o_out_b, net.tc_bias);
@@ -552,9 +653,11 @@ int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   return NM_OK;
 }
 
-template <bool kTrain, bool kView>
+template <bool kTrain, bool kView, bool kTime = false>
 static int launch_tc(nm_ctx* ctx, const TcParams& P, cudaStream_t st) {
-  auto kernel = kView ? k_mlp_tc<kTrain> : k_mlp_tc_noview<kTrain>;
+  void (*kernel)(const TcParams);
+  if constexpr (kTime) kernel = k_mlp_tc_nerft<kTrain>;
+  else kernel = kView ? k_mlp_tc<kTrain> : k_mlp_tc_noview<kTrain>;
   NM_SET_SMEM_ONCE(ctx, kernel, TcCfg::SMEM_BYTES);
   long long ctas = ctx->sm_count;
   if (P.n_tiles < ctas) ctas = P.n_tiles > 0 ? P.n_tiles : 1;
@@ -564,14 +667,14 @@ static int launch_tc(nm_ctx* ctx, const TcParams& P, cudaStream_t st) {
 }
 
 int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views, const float* origins,
-                  const float* dirs, const float* z, int64_t n, int32_t group, float* raw, cudaStream_t st,
+                  const float* dirs, const float* z, int64_t n, int32_t group, float t, float* raw, cudaStream_t st,
                   const NmTrainStash* stash) {
   if (!net.f16 || !net.tc_bias) NM_FAIL(ctx, NM_ERR_STATE, "nm_tc_forward: weights not packed");
-  const bool view = net.kind == NM_NET_VIEW;
+  const bool view = net.kind != NM_NET_NOVIEW, time = net.kind == NM_NET_NERFT;
   TcParams P;
   P.wimg = reinterpret_cast<const uint8_t*>(net.f16);
-  P.plan = make_plan(view);
-  P.in = NmMlpInput{pts, views, origins, dirs, z, (long long)n, group};
+  P.plan = make_plan(view, time);
+  P.in = NmMlpInput{pts, views, origins, dirs, z, (long long)n, group, t};
   P.pos_pe = NmPeSpec{net.desc.pos_pe_kind, net.desc.pos_n_freqs, net.f32 + net.o_pos_cyc};
   P.dir_pe = NmPeSpec{net.desc.dir_pe_kind, net.desc.dir_n_freqs, net.f32 + net.o_dir_cyc};
   P.raw = raw;
@@ -588,6 +691,7 @@ int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
         (view && (tc_make_store_map(&P.map_f, stash->f, 1, (uint64_t)n, 256) || tc_make_store_map(&P.map_v, stash->v, 1, (uint64_t)n, 128))))
       NM_FAIL(ctx, NM_ERR_CUDA, "nm_mlp_forward_train: cuTensorMapEncodeTiled failed");
   }
+  if (time) return stash ? launch_tc<true, true, true>(ctx, P, st) : launch_tc<false, true, true>(ctx, P, st);
   if (!view) return stash ? launch_tc<true, false>(ctx, P, st) : launch_tc<false, false>(ctx, P, st);
   return stash ? launch_tc<true, true>(ctx, P, st) : launch_tc<false, true>(ctx, P, st);
 }

@@ -272,6 +272,7 @@ __global__ void __launch_bounds__(BwCfg<false>::THREADS, 1) k_mlp_tc_bwd_noview(
 // Sources are the context-owned fp32 copies of the weights in the "Wt[k = input][n = output]" layout (api.cu)
 struct BwPackSrc {
   const float* wt[8]; const float* feat_t; const float* views_t;
+  int pos_k;                // width of the position encoding that precedes layer 5's hidden input (63, NeRF-T nets 84)
 };
 
 // slab k of the image: (step b, k-block kb); element (n = input channel, kk = output channel inside the k-block)
@@ -280,7 +281,7 @@ __device__ __forceinline__ float bw_src_weight(const BwPackSrc& S, int b, int n,
   if (b == 0) return S.views_t[(size_t)n * NM_VIEWS_HID + out];                 // views input = [feature(256), dir PE]
   if (b == 1) return S.feat_t[(size_t)n * 256 + out];
   const int l = 9 - b;                                                          // b = 2..8 -> layer 7..1
-  return S.wt[l][(size_t)((l == 5 ? NM_POS_PE : 0) + n) * 256 + out];           // layer 5 input = [PE(63), hidden]
+  return S.wt[l][(size_t)((l == 5 ? S.pos_k : 0) + n) * 256 + out];            // layer 5 input = [PE(63 / 84), hidden]
 }
 
 // view = false: the image of a view-independent net (b2..b8 only) and output_linear's [256][4] -> [4][256]
@@ -344,7 +345,7 @@ int nm_impl_pe_backward(nm_ctx* ctx, const NmNet& net, int which, const float* x
 
 int nm_tc_pack_bwd(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   // both buffers depend on the kind of the net: a slot that changed kind gets them at the new sizes
-  const bool view = net.kind == NM_NET_VIEW;
+  const bool view = net.kind != NM_NET_NOVIEW;
   const uint32_t image_bytes = (uint32_t)bw_slabs(view) * TC_SLAB_BYTES;
   const size_t wfloats = view ? 384 : 1024;
   if (net.f16_bwd && net.bwd_bytes != image_bytes) {
@@ -362,6 +363,7 @@ int nm_tc_pack_bwd(nm_ctx* ctx, NmNet& net, cudaStream_t st) {
   BwPackSrc S;
   for (int l = 0; l < 8; ++l) S.wt[l] = net.f32 + net.o_pts_w[l];
   S.feat_t = net.f32 + net.o_feat_w; S.views_t = net.f32 + net.o_views_w;
+  S.pos_k = net.f32_pos_k;
   const unsigned blocks = (unsigned)((image_bytes / 2 + 255) / 256);
   k_bw_pack<<<blocks, 256, 0, st>>>(S, image_bytes, view, net.f16_bwd, net.f32 + (view ? net.o_rgb_w : net.o_out_w), net.bw_wrgb);
   NM_CHECK_LAUNCH(ctx);
@@ -378,7 +380,7 @@ int nm_tc_backward(nm_ctx* ctx, NmNet& net, const float* d_raw, const float* sca
   BwParams P;
   P.wimg = reinterpret_cast<const uint8_t*>(net.f16_bwd);
   P.d_raw = d_raw; P.scale = scale;
-  const bool view = net.kind == NM_NET_VIEW;
+  const bool view = net.kind != NM_NET_NOVIEW;
   P.w_alpha = net.f32 + net.o_alpha_w;
   P.w_rgb = net.bw_wrgb;
   P.st_m = st_m;

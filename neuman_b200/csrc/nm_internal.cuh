@@ -12,14 +12,17 @@
 #define NM_WIDTH 256          // nerf_width  (options/options.py:55)
 #define NM_DEPTH 8            // nerf_depth  (options/options.py:54)
 #define NM_POS_PE 63          // 3 + 3*2*10  (models/vanilla.py:60-79)
+#define NM_POS_PE_T 84        // 4 + 4*2*10: position encoding of a NeRF-T net, (x, y, z, t) (train.py:254-256)
 #define NM_DIR_PE 27          // 3 + 3*2*4
 #define NM_VIEWS_HID 128      // width/2     (models/vanilla.py:112)
 #define NM_RANGE_FLAG_WORD 32  // word of ctx->d_counter the tensor-core kernels OR their range flag into
 
 // ---- packed network ------------------------------------------------------------------------
 // Net kinds: NeRF with use_viewdirs=True (alpha / feature / views / rgb heads, nm_net_pack) or use_viewdirs=False
-// (one output_linear [4,256] on layer 7, no direction input, nm_net_pack_noview; models/vanilla.py:117-118,145-146).
-enum { NM_NET_VIEW = 0, NM_NET_NOVIEW = 1 };
+// (one output_linear [4,256] on layer 7, no direction input, nm_net_pack_noview; models/vanilla.py:117-118,145-146),
+// or a view-dependent NeRF-T net whose position input carries the time as a fourth column (--ablate_nerft,
+// nm_net_pack_nerft; rendered and trained, no input gradients).
+enum { NM_NET_VIEW = 0, NM_NET_NOVIEW = 1, NM_NET_NERFT = 2 };
 
 // fp32 transposed weights ([in_padded][out]) for the SIMT kernel live in one device allocation per slot; the
 // tensor-core kernels read fp16 slabs in the 128B-swizzled wgmma layout from their own allocations.
@@ -30,6 +33,7 @@ struct NmNet {
   // SIMT fp32 layout: Wt[k][n] (k = input index, n = output index), biases as given
   float* f32 = nullptr;             // base allocation
   size_t f32_floats = 0;
+  int f32_pos_k = 0;                // position-encoding width the f32 layout is sized for (NM_POS_PE or NM_POS_PE_T)
   // offsets (in floats) into f32
   size_t o_pts_w[8], o_pts_b[8], o_feat_w, o_feat_b, o_alpha_w, o_alpha_b, o_views_w, o_views_b,
       o_rgb_w, o_rgb_b, o_pos_bv, o_dir_bv, o_pos_cyc, o_dir_cyc,
@@ -187,10 +191,13 @@ int nm_impl_raygen(nm_ctx* ctx, const nm_camera* cam, int mode, int64_t pix0, in
 // composite.cu: raw2outputs whose last sample is followed by zero-density samples starting at z_end
 int nm_impl_raw2outputs_zend(nm_ctx* ctx, const float* raw, const float* z, const float* rays_d, int64_t R, int32_t S,
                              int32_t white_bkg, float z_end, float* rgb, float* depth, cudaStream_t st);
+// api.cu: nm_mlp_forward_rays with the time of every sample (t, read by NeRF-T slots only)
+int nm_impl_mlp_forward_rays(nm_ctx* ctx, int slot, int mode, const float* origins, const float* dirs, const float* z,
+                             int64_t R, int32_t S, float t, float* raw, cudaStream_t st);
 // mlp_simt.cu
 int nm_simt_forward(nm_ctx* ctx, const NmNet& net, const float* pts, const float* views,
                     const float* origins, const float* dirs, const float* z, int64_t n,
-                    int32_t group, float* raw, cudaStream_t st);
+                    int32_t group, float t, float* raw, cudaStream_t st);
 // mlp_tc.cu
 int nm_tc_pack(nm_ctx* ctx, NmNet& net, cudaStream_t st);
 // fp16 activation stash written by the training forward and read by the backward chain (mlp_tc_bwd.cu)
@@ -210,4 +217,4 @@ int nm_tc_backward(nm_ctx* ctx, NmNet& net, const float* d_raw, const float* sca
                    const uint32_t* st_m, __half* g_pre, __half* g_f, __half* g_v, cudaStream_t st);
 int nm_tc_forward(nm_ctx* ctx, NmNet& net, const float* pts, const float* views,
                   const float* origins, const float* dirs, const float* z, int64_t n,
-                  int32_t group, float* raw, cudaStream_t st, const NmTrainStash* stash = nullptr);
+                  int32_t group, float t, float* raw, cudaStream_t st, const NmTrainStash* stash = nullptr);

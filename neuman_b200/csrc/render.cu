@@ -122,9 +122,13 @@ int check_frame(nm_ctx* ctx, const nm_camera* cam, const nm_render_opts* opt, in
   return NM_OK;
 }
 
-int check_slot(nm_ctx* ctx, int slot, const char* who) {
+// `nerft`: the driver takes a frame time and needs NeRF-T nets (nm_render_vanilla_t); every other driver takes no time
+// and refuses them (the reference's hybrid renderers have no NeRF-T path)
+int check_slot(nm_ctx* ctx, int slot, const char* who, bool nerft = false) {
   if (slot < 0 || slot >= NM_MAX_NET_SLOTS || !ctx->nets[slot].packed)
     NM_FAIL(ctx, NM_ERR_STATE, std::string(who) + ": net slot not packed");
+  if ((ctx->nets[slot].kind == NM_NET_NERFT) != nerft)
+    NM_FAIL(ctx, NM_ERR_UNSUPPORTED, std::string(who) + (nerft ? ": needs NeRF-T nets" : ": NeRF-T nets need the frame time (nm_render_vanilla_t)"));
   return NM_OK;
 }
 
@@ -176,19 +180,20 @@ int render_frame(nm_ctx* ctx, const nm_camera* cam, const nm_render_opts* opt, i
 }
 
 // background coarse (+fine) pass over C rays already in o/d: leaves raw/z of the last pass in
-// (*raw_out, *z_out) with *S_out samples.  utils/render_utils.py:141-153 / :287-298 / :398-409
+// (*raw_out, *z_out) with *S_out samples.  utils/render_utils.py:141-153 / :287-298 / :398-409.  t: the time of every
+// sample, read by NeRF-T nets only (:134-137)
 int bkg_pass(nm_ctx* ctx, int coarse, int fine, const nm_render_opts* opt, const float* o, const float* d, int64_t C,
              float* z_c, float* raw_c, float* w_c, float* z_f, float* raw_f, float** raw_out, float** z_out,
-             int* S_out, cudaStream_t st) {
+             int* S_out, cudaStream_t st, float t = 0.f) {
   const int S = opt->samples_per_ray, N = opt->importance_samples_per_ray;
   TRY(nm_ray_to_samples(ctx, o, d, nullptr, nullptr, opt->near_bkg, opt->far_bkg, C, S, 0, nullptr, nullptr, nullptr,
                         z_c, st));
-  TRY(nm_mlp_forward_rays(ctx, coarse, opt->mlp_mode, o, d, z_c, C, S, raw_c, st));
+  TRY(nm_impl_mlp_forward_rays(ctx, coarse, opt->mlp_mode, o, d, z_c, C, S, t, raw_c, st));
   ctx->last_mlp_evals += C * S;
   if (fine >= 0 && N > 0) {
     TRY(nm_raw2outputs(ctx, raw_c, z_c, d, C, S, nullptr, 1.f, opt->white_bkg, nullptr, nullptr, nullptr, w_c, nullptr, st));
     TRY(nm_importance_samples(ctx, o, d, z_c, w_c, C, S, N, 1, nullptr, nullptr, z_f, st));
-    TRY(nm_mlp_forward_rays(ctx, fine, opt->mlp_mode, o, d, z_f, C, S + N, raw_f, st));
+    TRY(nm_impl_mlp_forward_rays(ctx, fine, opt->mlp_mode, o, d, z_f, C, S + N, t, raw_f, st));
     ctx->last_mlp_evals += C * (S + N);
     *raw_out = raw_f; *z_out = z_f; *S_out = S + N;
   } else {
@@ -262,17 +267,13 @@ int human_branch(nm_ctx* ctx, int slot, const nm_render_opts* opt, const float* 
   return NM_OK;
 }
 
-}  // namespace
-
-// ---------------------------------------------------------------------------------------------
-extern "C" int nm_render_vanilla(nm_ctx* ctx, int coarse_slot, int fine_slot, const nm_camera* cam,
-                                 const nm_render_opts* opt, int64_t pix0, int64_t n, const int32_t* pixels, float* rgb,
-                                 float* depth, int32_t host_out, void* stream) {
-  NM_ENTER(ctx);
-  TRY(check_frame(ctx, cam, opt, pix0, n, pixels, rgb, __func__));
-  TRY(check_slot(ctx, coarse_slot, __func__));
-  if (fine_slot >= 0) TRY(check_slot(ctx, fine_slot, __func__));
-  cudaStream_t st = (cudaStream_t)stream;
+// nm_render_vanilla and nm_render_vanilla_t (nerft: NeRF-T nets, every sample at time t)
+int render_vanilla(nm_ctx* ctx, int coarse_slot, int fine_slot, const nm_camera* cam, const nm_render_opts* opt, bool nerft,
+                   float t, int64_t pix0, int64_t n, const int32_t* pixels, float* rgb, float* depth, int32_t host_out,
+                   cudaStream_t st, const char* who) {
+  TRY(check_frame(ctx, cam, opt, pix0, n, pixels, rgb, who));
+  TRY(check_slot(ctx, coarse_slot, who, nerft));
+  if (fine_slot >= 0) TRY(check_slot(ctx, fine_slot, who, nerft));
   const int S = opt->samples_per_ray, N = fine_slot >= 0 ? opt->importance_samples_per_ray : 0;
   float *z_c, *raw_c, *w_c, *z_f, *raw_f;
   return render_frame(ctx, cam, opt, 1, pix0, n, pixels, Planes{rgb, depth, nullptr}, host_out, st,   // shot_all_rays (:122)
@@ -282,9 +283,28 @@ extern "C" int nm_render_vanilla(nm_ctx* ctx, int coarse_slot, int fine_slot, co
     },
     [&](int64_t c, const float* o, const float* d, const Planes& dst) -> int {
       float *raw, *z; int St;
-      TRY(bkg_pass(ctx, coarse_slot, fine_slot, opt, o, d, c, z_c, raw_c, w_c, z_f, raw_f, &raw, &z, &St, st));
+      TRY(bkg_pass(ctx, coarse_slot, fine_slot, opt, o, d, c, z_c, raw_c, w_c, z_f, raw_f, &raw, &z, &St, st, t));
       return nm_raw2outputs(ctx, raw, z, d, c, St, nullptr, 1.f, opt->white_bkg, dst.rgb, nullptr, nullptr, nullptr, dst.depth, st);
     });
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------
+extern "C" int nm_render_vanilla(nm_ctx* ctx, int coarse_slot, int fine_slot, const nm_camera* cam,
+                                 const nm_render_opts* opt, int64_t pix0, int64_t n, const int32_t* pixels, float* rgb,
+                                 float* depth, int32_t host_out, void* stream) {
+  NM_ENTER(ctx);
+  return render_vanilla(ctx, coarse_slot, fine_slot, cam, opt, false, 0.f, pix0, n, pixels, rgb, depth, host_out,
+                        (cudaStream_t)stream, __func__);
+}
+
+extern "C" int nm_render_vanilla_t(nm_ctx* ctx, int coarse_slot, int fine_slot, const nm_camera* cam,
+                                   const nm_render_opts* opt, float frame_time, int64_t pix0, int64_t n,
+                                   const int32_t* pixels, float* rgb, float* depth, int32_t host_out, void* stream) {
+  NM_ENTER(ctx);
+  return render_vanilla(ctx, coarse_slot, fine_slot, cam, opt, true, frame_time, pix0, n, pixels, rgb, depth, host_out,
+                        (cudaStream_t)stream, __func__);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -39,9 +39,12 @@ def supported_joiner(j):
     """True when `j` is a Joiner the kernels implement: 8x256 trunk, skip after layer 4, no output scaling, 10
     log-spaced position frequencies with the input included, 'posenc' or 'rotate' mapping, and either view directions
     (4 direction frequencies, same conditions) or no view directions with output_linear [4,256] (use_viewdirs=False:
-    the direction encoding is never used)."""
+    the direction encoding is never used).  A NeRF-T net (--ablate_nerft: position input (x, y, z, t)) qualifies with
+    view directions and the 'posenc' position mapping."""
     try:
         n, pp = j.nerf, j.pos_pe
+        if pp.input_dims == 4 and (not n.use_viewdirs or pp.mapping != "posenc"):
+            return False
         if not n.use_viewdirs:
             return bool(len(n.pts_linears) == 8 and tuple(n.skips) == (4,)
                         and tuple(n.pts_linears[1].weight.shape) == (256, 256)
@@ -53,7 +56,7 @@ def supported_joiner(j):
         return bool(n.use_viewdirs and len(n.pts_linears) == 8 and tuple(n.skips) == (4,)
                     and tuple(n.pts_linears[1].weight.shape) == (256, 256)
                     and getattr(n, "scale_type", "no") == "no"
-                    and pp.N_freqs == 10 and dp.N_freqs == 4 and pp.input_dims == 3 and dp.input_dims == 3
+                    and pp.N_freqs == 10 and dp.N_freqs == 4 and pp.input_dims in (3, 4) and dp.input_dims == 3
                     and pp.log_sampling and dp.log_sampling and pp.include_input and dp.include_input
                     and pp.mapping in ("posenc", "rotate") and dp.mapping in ("posenc", "rotate")
                     and float(dp.max_freq) == 3.0 and float(getattr(dp, "min_freq", 0)) == 0.0)
@@ -96,8 +99,8 @@ def install(reference_root=None, train=False):
                 and supported_joiner(self):
             if not torch.is_grad_enabled():
                 return ops.joiner_forward(self, input_pts, input_views)
-            if train:
-                return autograd.joiner_forward(self, input_pts, input_views)
+            if train and not (ops.is_nerft(self) and (input_pts.requires_grad or input_views.requires_grad)):
+                return autograd.joiner_forward(self, input_pts, input_views)   # (no input gradients for NeRF-T nets)
         return ref_forward(self, input_pts, input_views)          # other training / CPU / other architectures
     mv.Joiner.forward = joiner_forward
 
@@ -139,13 +142,18 @@ def install(reference_root=None, train=False):
         return [model.coarse_bkg_net, model.fine_bkg_net] + [h.coarse_human_net for h in humans]
 
     def supported_call(name, model, a, k):
+        # render_vanilla(ablate_nerft=True) renders NeRF-T nets at the frame's time; every other call takes plain nets
+        nerft = name == "render_vanilla" and bool(k.get("ablate_nerft", False))
         try:
             nets = nets_of(name, model, a, k)
-            if not all(next(n.parameters()).is_cuda and supported_joiner(n) for n in nets):
+            if not all(next(n.parameters()).is_cuda and supported_joiner(n) and ops.is_nerft(n) == nerft for n in nets):
                 return False
-        except (AttributeError, StopIteration, TypeError):
+            if nerft:
+                cap = k.get("cap", a[0] if a else None)
+                float(cap.frame_id["frame_id"]) / float(cap.frame_id["total_frames"])
+        except (AttributeError, StopIteration, TypeError, KeyError, ZeroDivisionError):
             return False
-        return not k.get("ablate_nerft", False)
+        return not k.get("ablate_nerft", False) or nerft
 
     for name in ("render_vanilla", "render_smpl_nerf", "render_hybrid_nerf", "render_hybrid_nerf_multi_persons"):
         ref_fn, new_fn = o_ru[name], getattr(render, name)
@@ -167,16 +175,20 @@ def install(reference_root=None, train=False):
     def constants_of_the_step(*ts):
         return on_cuda(*ts) and (not torch.is_grad_enabled() or train)
 
+    def time_ok(append_t):
+        # the time column is concatenated as given (:133-134): any tensor that is a constant of the step
+        return append_t is None or (isinstance(append_t, torch.Tensor) and not append_t.requires_grad)
+
     def ray_to_samples(ray_batch, samples_per_ray, lindisp=False, perturb=0., device='cpu', append_t=None):
-        if append_t is None and constants_of_the_step(ray_batch['origin'], ray_batch['near']):
-            return ops.ray_to_samples(ray_batch, samples_per_ray, lindisp, perturb)
+        if time_ok(append_t) and constants_of_the_step(ray_batch['origin'], ray_batch['near']):
+            return ops.ray_to_samples(ray_batch, samples_per_ray, lindisp, perturb, append_t=append_t)
         return ref_rts(ray_batch, samples_per_ray, lindisp, perturb, device, append_t)
 
     def ray_to_importance_samples(ray_batch, z_vals, weights, importance_samples_per_ray, device='cpu',
                                   including_old=True, append_t=None):
-        if append_t is None and constants_of_the_step(z_vals, weights):       # samples are constants of the step (:150 detaches)
+        if time_ok(append_t) and constants_of_the_step(z_vals, weights):       # samples are constants of the step (:150 detaches)
             return ops.ray_to_importance_samples(ray_batch, z_vals, weights, importance_samples_per_ray,
-                                                 including_old=including_old)
+                                                 including_old=including_old, append_t=append_t)
         return ref_rtis(ray_batch, z_vals, weights, importance_samples_per_ray, device, including_old, append_t)
 
     def sample_pdf(bins, weights, N_samples, det=False, device='cpu'):

@@ -90,11 +90,19 @@ def is_viewless(joiner):
     return not getattr(joiner.nerf, "use_viewdirs", True)
 
 
+def is_nerft(joiner):
+    """True for a NeRF-T net (the reference's --ablate_nerft background nets): its position input is (x, y, z, t)."""
+    return int(getattr(joiner.pos_pe, "input_dims", 3)) == 4
+
+
 def net_slot(joiner, ctx=None):
     """Packs (lazily, keyed on a per-module uid + parameter storage + version) a Joiner into a library slot: a
     view-dependent net (use_viewdirs=True) with nm_net_pack, a view-independent one (use_viewdirs=False, output_linear
-    [4,256]) with nm_net_pack_noview."""
+    [4,256]) with nm_net_pack_noview, a NeRF-T net (4-D posenc position input, view-dependent) with nm_net_pack_nerft."""
     nerf = joiner.nerf
+    viewless, nerft = is_viewless(joiner), is_nerft(joiner)
+    if nerft and (viewless or joiner.pos_pe.mapping != "posenc"):
+        raise NotImplementedError("NeRF-T nets: only view-dependent nets with the posenc position mapping are built")
     p0 = nerf.pts_linears[0].weight
     ctx = ctx or _ctx_for(p0)
     key = _net_key(joiner)
@@ -103,7 +111,6 @@ def net_slot(joiner, ctx=None):
         ctx.slot_clock += 1
         ctx.slot_used[s] = ctx.slot_clock
         return s
-    viewless = is_viewless(joiner)
     if viewless and tuple(nerf.output_linear.weight.shape) != (4, 256):
         raise NotImplementedError("view-independent nets: only output_linear [4,256] (output_ch=4) is built")
     if viewless and getattr(nerf, "scale_type", "no") != "no":
@@ -147,7 +154,8 @@ def net_slot(joiner, ctx=None):
         dp = joiner.dir_pe
         d.dir_pe_kind = _PE_KIND[dp.mapping]
         d.dir_min_freq, d.dir_max_freq, d.dir_n_freqs = float(dp.min_freq), float(dp.max_freq), int(dp.N_freqs)
-        ctx.check(ctx.lib.nm_net_pack(ctx.h, s, C.byref(d), ctx.stream()))
+        pack = ctx.lib.nm_net_pack_nerft if nerft else ctx.lib.nm_net_pack
+        ctx.check(pack(ctx.h, s, C.byref(d), ctx.stream()))
     if keep:
         torch.cuda.current_stream(ctx.device).synchronize()  # `keep` temporaries may be freed after this
     ctx.slots[key] = s
@@ -159,14 +167,14 @@ def net_slot(joiner, ctx=None):
 
 def joiner_forward(joiner, input_pts, input_views=None, mode=None):
     """Joiner.forward (models/vanilla.py:162-166) -> [...,4].  A view-independent net ignores input_views (may be None),
-    as the reference does (:145-146)."""
+    as the reference does (:145-146); a NeRF-T net takes input_pts [...,4] = (x, y, z, t)."""
     viewless = is_viewless(joiner)
     if input_views is None and not viewless:
         raise NotImplementedError("use_viewdirs=True networks need input_views")
     ctx = _ctx_for(input_pts)
     slot = net_slot(joiner, ctx)
     shape = input_pts.shape[:-1]
-    pts = _f32(input_pts).reshape(-1, 3)
+    pts = _f32(input_pts).reshape(-1, 4 if is_nerft(joiner) else 3)
     views = None
     if not viewless:
         views = _f32(input_views, pts.device).reshape(-1, 3)
@@ -262,9 +270,8 @@ def near_far_mesh(orig, dir, actor, geo_threshold=DEFAULT_GEO_THRESH):
 
 
 def ray_to_samples(ray_batch, samples_per_ray, lindisp=False, perturb=0., device='cuda', append_t=None, t_rand=None):
-    """utils/ray_utils.py:96-135 -> (pts [R,S,3], dirs [R,S,3], z_vals [R,S])."""
-    if append_t is not None:
-        raise NotImplementedError("append_t (ablate_nerft) is not on the built path")
+    """utils/ray_utils.py:96-135 -> (pts [R,S,3], dirs [R,S,3], z_vals [R,S]); with append_t [R,S,1] the time column is
+    concatenated to pts ([R,S,4]) as the reference does (:133-134)."""
     o = _f32(ray_batch['origin'])
     ctx = _ctx_for(o)
     d = _f32(ray_batch['direction'], o.device)
@@ -281,6 +288,8 @@ def ray_to_samples(ray_batch, samples_per_ray, lindisp=False, perturb=0., device
         tr = _f32(t_rand, o.device) if t_rand is not None else torch.rand(R, S, device=o.device)
     ctx.check(ctx.lib.nm_ray_to_samples(ctx.h, _p(o), _p(d), _p(near), _p(far), 0.0, 0.0, R, S, int(bool(lindisp)),
                                         _p(tr), _p(pts), _p(dirs), _p(z), ctx.stream()))
+    if append_t is not None:
+        pts = torch.cat([pts, append_t.to(pts.device)], dim=-1)
     return pts, dirs, z
 
 
@@ -301,9 +310,7 @@ def sample_pdf(bins, weights, N_samples, det=False, device='cuda', u=None):
 
 def ray_to_importance_samples(ray_batch, z_vals, weights, importance_samples_per_ray, device='cuda',
                               including_old=True, append_t=None):
-    """utils/ray_utils.py:138-160."""
-    if append_t is not None:
-        raise NotImplementedError("append_t (ablate_nerft) is not on the built path")
+    """utils/ray_utils.py:138-160 (append_t: as ray_to_samples, :158-159)."""
     z = _f32(z_vals)
     ctx = _ctx_for(z)
     o, d = _f32(ray_batch['origin'], z.device), _f32(ray_batch['direction'], z.device)
@@ -316,6 +323,8 @@ def ray_to_importance_samples(ray_batch, z_vals, weights, importance_samples_per
     zo = torch.empty(R, total, device=z.device)
     ctx.check(ctx.lib.nm_importance_samples(ctx.h, _p(o), _p(d), _p(z), _p(w), R, S, N, int(bool(including_old)),
                                             _p(pts), _p(dirs), _p(zo), ctx.stream()))
+    if append_t is not None:
+        pts = torch.cat([pts, append_t.to(pts.device)], dim=-1)
     return pts, dirs, zo
 
 

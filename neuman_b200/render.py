@@ -98,14 +98,18 @@ def _render(device, cap, pix0, n, pixels, out, host_out, planes, driver):
 
 def render_vanilla_range(coarse_net, cap, fine_net=None, samples_per_ray=64, importance_samples_per_ray=128,
                          white_bkg=True, near_far_source='bkg', pix0=0, n=None, host_out=True, chunk=CHUNK, pixels=None,
-                         out=None):
+                         out=None, frame_time=None):
     """Renders the row-major pixel range [pix0, pix0+n), or the pixel list `pixels` (int32 CUDA tensor). host_out: pinned
-    host tensors (device->host copy inside the call) else CUDA tensors. Returns (rgb [n,3], depth [n])."""
+    host tensors (device->host copy inside the call) else CUDA tensors. frame_time: NeRF-T nets, the time of every
+    sample (nm_render_vanilla_t). Returns (rgb [n,3], depth [n])."""
     def driver(ctx, cam, n, pix, rgb, depth):
         cs = ops.net_slot(coarse_net, ctx)
         fs = ops.net_slot(fine_net, ctx) if fine_net is not None else -1
         o = _opts(samples_per_ray, importance_samples_per_ray if fine_net is not None else 0, white_bkg,
                   cap.near[near_far_source], cap.far[near_far_source], chunk=chunk)
+        if frame_time is not None:
+            return ctx.lib.nm_render_vanilla_t(ctx.h, cs, fs, C.byref(cam), C.byref(o), float(frame_time), pix0, n, pix, rgb,
+                                               depth, int(host_out), ctx.stream())
         return ctx.lib.nm_render_vanilla(ctx.h, cs, fs, C.byref(cam), C.byref(o), pix0, n, pix, rgb, depth, int(host_out),
                                          ctx.stream())
     return _render(_device_of(coarse_net), cap, pix0, n, pixels, out, host_out, 2, driver)
@@ -114,11 +118,13 @@ def render_vanilla_range(coarse_net, cap, fine_net=None, samples_per_ray=64, imp
 def render_vanilla(coarse_net, cap, fine_net=None, rays_per_batch=32768, samples_per_ray=64,
                    importance_samples_per_ray=128, white_bkg=True, near_far_source='bkg', return_depth=False,
                    ablate_nerft=False):
-    """utils/render_utils.py:108-161."""
+    """utils/render_utils.py:108-161.  ablate_nerft: NeRF-T nets, rendered at the frame's time frame_id / total_frames
+    in float32 (what `torch.ones(...) * cur_time` holds, :135-137)."""
+    t = None
     if ablate_nerft:
-        raise NotImplementedError("ablate_nerft is not on the built path")
+        t = float(np.float32(cap.frame_id['frame_id'] / cap.frame_id['total_frames']))
     rgb, depth = render_vanilla_range(coarse_net, cap, fine_net, samples_per_ray, importance_samples_per_ray, white_bkg,
-                                      near_far_source)
+                                      near_far_source, frame_time=t)
     H, W = cap.shape
     rgb = rgb.numpy().reshape(H, W, 3)
     if return_depth:

@@ -18,15 +18,20 @@ def vanilla_loss_func(coarse_net, fine_net, batch, opt, penalize_empty_space=0.,
     (and depth [R] when penalize_empty_space > 0).  Returns the reference's four losses.
     `t_rand` / `noise` = (coarse, fine) pairs let a test fix the stratified jitter and the density noise.
     `check_bad_weights` keeps the reference's dead-density re-initialisation (:84-89); it costs one host
-    sync per step, pass False to run the step fully asynchronously."""
-    if getattr(opt, 'ablate_nerft', False):
-        raise NotImplementedError("ablate_nerft is not on the built path")
+    sync per step, pass False to run the step fully asynchronously.
+    opt.ablate_nerft: NeRF-T nets; every sample carries its ray's time batch['viewf_list'] [R,1] as a fourth position
+    column (:47-50)."""
     dev = next(coarse_net.parameters()).device
+    coarse_time = fine_time = None
+    if getattr(opt, 'ablate_nerft', False):
+        tv = batch['viewf_list'].to(dev).reshape(-1, 1)
+        coarse_time = tv.repeat(1, opt.samples_per_ray)[..., None]
+        fine_time = tv.repeat(1, opt.samples_per_ray + opt.importance_samples_per_ray)[..., None]
     perturb = getattr(opt, 'perturb', 0.)
     noise_std = getattr(opt, 'raw_noise_std', 0.)
     color = batch['color'].to(dev)
     pts, dirs, z_vals = ops.ray_to_samples(batch, opt.samples_per_ray, perturb=perturb, device=dev,
-                                           t_rand=t_rand)
+                                           t_rand=t_rand, append_t=coarse_time)
     _b, _n = z_vals.shape
     out = coarse_net(pts, dirs)
     rgb_map, _, _, weights, _ = autograd.raw2outputs(out, z_vals, dirs[:, 0, :], raw_noise_std=noise_std,
@@ -41,7 +46,7 @@ def vanilla_loss_func(coarse_net, fine_net, batch, opt, penalize_empty_space=0.,
     fine_rgb_loss, fine_empty, F_out = torch.zeros_like(coarse_rgb_loss), torch.zeros_like(coarse_rgb_loss), None
     if fine_net is not None:
         F_pts, F_dirs, F_z = ops.ray_to_importance_samples(batch, z_vals, weights.detach(),
-                                                           opt.importance_samples_per_ray, device=dev)
+                                                           opt.importance_samples_per_ray, device=dev, append_t=fine_time)
         F_out = fine_net(F_pts, F_dirs)
         F_rgb, _, _, _, _ = autograd.raw2outputs(F_out, F_z, F_dirs[:, 0, :], raw_noise_std=noise_std,
                                                  white_bkg=opt.white_bkg, noise=None if noise is None else noise[1])
