@@ -25,10 +25,12 @@
 // ---------------------------------------------------------------------------------------------
 // Plan: which slabs a step consumes, where they live in the packed image.
 // ---------------------------------------------------------------------------------------------
+#define TC_MAX_SLABS 64
 struct TcPlan {
   uint32_t slab_off[TC_STEPS][6];   // byte offset inside the image
   uint32_t slab_bytes[TC_STEPS];    // bytes per slab of this step
   uint32_t image_bytes;             // size of the image
+  uint32_t lin_off[TC_MAX_SLABS + 1];   // offset of the j-th slab in consumption order (= image order); [slabs] = image_bytes
 };
 
 // Every layer's bias rides in the MMAs.  The last channel of each encoding is the constant 1 (channel 63 of the position
@@ -64,6 +66,7 @@ __host__ __device__ constexpr int tc_slabs_per_tile(bool v = true, bool t = fals
   for (int s = 0; s < tc_steps(v); ++s) n += step_nkb(s, v, t);
   return n;
 }
+static_assert(tc_slabs_per_tile(true, true) <= TC_MAX_SLABS && tc_slabs_per_tile(true) <= TC_MAX_SLABS, "slab table too small");
 
 struct TcCfg {
   static constexpr int THREADS = 256;                  // two consumer warpgroups
@@ -276,26 +279,28 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
   for (int i = threadIdx.x; i < TC_CONST_FLOATS; i += C::THREADS) s_const[i] = __ldg(P.consts + i);
   const long long my_tiles = blockIdx.x < P.n_tiles ? (P.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
   const uint32_t total = (uint32_t)(my_tiles * SLABS);
-  // producer state (thread 0): next slab to issue and its (step, k-block)
-  uint32_t pq = 0;
-  int ps = 0, pkb = 0;
-  auto produce = [&]() {
-    if (pq >= total) return;
-    if (pq >= TC_NSLOT) mbar_wait(R.empty(pq), (pq / TC_NSLOT - 1) & 1);
-    const uint32_t bytes = P.plan.slab_bytes[ps];
-    mbar_arrive_expect_tx(R.full(pq), bytes);
-    bulk_g2s(R.slot(pq), P.wimg + P.plan.slab_off[ps][pkb], bytes, R.full(pq));
-    ++pq;
-    if (++pkb == step_nkb(ps, kView, kTime)) { pkb = 0; if (++ps == STEPS) ps = 0; }
+  // Refills: the warpgroup that releases a slot second issues the slab TC_NSLOT places further on, right away.  A
+  // per-slot release counter in place of an `empty` barrier decides which one that is, so neither warpgroup ever waits
+  // for the other's release: warpgroup 0 keeps issuing MMAs on the slabs already in the ring while warpgroup 1 is behind
+  // (e.g. in its epilogue), and the other way round.
+  const uint32_t rel = sbase + C::OFF_BAR + 8 * TC_NSLOT;          // TC_NSLOT release counters (u32)
+  auto refill = [&](uint32_t qq) {
+    const uint32_t j = qq % SLABS, off = P.plan.lin_off[j], bytes = P.plan.lin_off[j + 1] - off;
+    mbar_arrive_expect_tx(R.full(qq), bytes);
+    bulk_g2s(R.slot(qq), P.wimg + off, bytes, R.full(qq));
   };
   if (threadIdx.x == 0) {
-    R.init();
-    for (int i = 0; i < TC_NSLOT; ++i) produce();
+    for (int i = 0; i < TC_NSLOT; ++i) {
+      mbar_init(R.full(i), 1);
+      st_shared_u32(rel + 4 * i, 0);
+    }
+    fence_mbar_init();
+    for (uint32_t i = 0; i < TC_NSLOT && i < total; ++i) refill(i);
   }
   __syncthreads();
   auto release = [&](uint32_t qq) {
-    if (wtid == 0) mbar_arrive_local(R.empty(qq));
-    if (threadIdx.x == 0) produce();
+    // acq_rel: the first releaser's finished MMA reads of the slot are ordered before the second one's refill
+    if (wtid == 0 && qq + TC_NSLOT < total && (atom_add_acq_rel_cta(rel + 4 * (qq % TC_NSLOT), 1) & 1)) refill(qq + TC_NSLOT);
     __syncwarp();
   };
 
@@ -620,11 +625,15 @@ int nm_tc_encode(nm_ctx* ctx, const NmNet& net, int which, const float* x, int64
 static TcPlan make_plan(bool view, bool time) {
   TcPlan p{};
   uint32_t off = 0;
+  int j = 0;
   for (int s = 0; s < tc_steps(view); ++s) {
     p.slab_bytes[s] = (uint32_t)step_N(s, view) * 128u;
-    for (int kb = 0; kb < step_nkb(s, view, time); ++kb) { p.slab_off[s][kb] = off; off += p.slab_bytes[s]; }
+    for (int kb = 0; kb < step_nkb(s, view, time); ++kb) {
+      p.slab_off[s][kb] = p.lin_off[j++] = off;
+      off += p.slab_bytes[s];
+    }
   }
-  p.image_bytes = off;
+  p.lin_off[j] = p.image_bytes = off;
   return p;
 }
 

@@ -29,6 +29,15 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "DONE:\n\t"
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+// returns the old value
+__device__ __forceinline__ uint32_t atom_add_acq_rel_cta(uint32_t addr, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(addr), "r"(v) : "memory");
+  return old;
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -181,8 +190,9 @@ __device__ __forceinline__ void tma_store_rows(const CUtensorMap* map, uint32_t 
 }
 
 // One warpgroup's view of the weight ring: the slabs of a launch are consumed in a fixed order by both warpgroups; a slab's
-// slot is refilled once both have released it.  Thread 0 of the CTA is the producer: it issues the first TC_NSLOT slabs
-// and, after each of its own releases, the slab TC_NSLOT places further on.
+// slot is refilled once both have released it.  In the backward chain thread 0 of the CTA is the producer: it issues the
+// first TC_NSLOT slabs and, after each of its own releases, waits on `empty` and issues the slab TC_NSLOT places further
+// on.  The forward kernel (mlp_tc.cu) uses the slots and `full` barriers only: there the second releaser refills.
 struct TcRing {
   uint32_t ring, bar;       // shared addresses: TC_NSLOT slots of TC_SLAB_BYTES; full[TC_NSLOT] then empty[TC_NSLOT]
   __device__ uint32_t slot(uint32_t q) const { return ring + (q % TC_NSLOT) * TC_SLAB_BYTES; }
