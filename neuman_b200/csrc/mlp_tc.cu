@@ -1,23 +1,27 @@
 // Tensor-core implementation of Joiner.forward (positional encoding + 8x256 NeRF MLP,
-// models/vanilla.py:82-92,:120-152,:162-166) for sm_90a: wgmma (fp16 operands from shared memory, fp32
-// accumulators in registers), weights streamed by bulk-TMA (cp.async.bulk) through a shared-memory ring,
-// activations kept on chip between layers, persistent CTAs.
+// models/vanilla.py:82-92,:120-152,:162-166) for sm_90a: wgmma (fp16 operands, fp32 accumulators in registers),
+// weights streamed by bulk-TMA (cp.async.bulk) through a shared-memory ring, activations kept in registers between
+// layers, persistent CTAs.
 //
 // fp16 operands carry the same 11-bit significand as TF32, at twice the tensor rate; accumulation,
 // bias, ReLU, the alpha head and the encodings are fp32 (DESIGN.md "Numerics").
 //
 // Work decomposition
 //   tile      = 128 consecutive samples per CTA, 64 per consumer warpgroup (wgmma M = 64).  The two warpgroups
-//               share every weight slab; each has its own activation buffer and encodings.
+//               share every weight slab; each has its own activations and encodings.
 //   step      = one GEMM of the network: 0: L0 (K=64 PE) | 1-4: L1-4 | 5: L5 (PE block + 4 act
 //               blocks, "input first", :131) | 6,7: L6,L7 (+alpha head in the epilogue of 7, :135) |
 //               8: feature (:136) | 9: views layer (4 feature blocks + dir-PE block, N=128, :137-141) |
 //               10: rgb (N=16, 3 used, :143).
 //   slab      = one 64-wide K block of one step's weights: [N rows][128 B], 128B-swizzled, K-major -- the GMMA
 //               canonical layout, pre-packed in HBM so one cp.async.bulk moves it.  Slabs flow through a
-//               TC_NSLOT-deep ring (tc_common.cuh: TcRing).
-//   epilogue  : accumulator registers -> ReLU -> cvt to f16x2 -> swizzled st.shared into the warpgroup's
-//               activation buffer, which is the next step's A operand (in place).
+//               TcCfg::NSLOT-deep ring (tc_common.cuh: TcRing): 4 slots, 6 in the view-independent render kernel.
+//   epilogue  : accumulator registers -> ReLU -> cvt to f16x2 -> `a`, the A register fragments of the next step's
+//               MMAs (the accumulator layout of 16 columns is the A fragment layout of one K = 16 slice).  The
+//               training forward also writes the swizzled activation block in shared memory, the source of the
+//               stash's TMA stores.  A step's k-blocks: the position encoding from shared memory (steps 0 and 5),
+//               the activation k-blocks from `a`, then one from shared memory (bias slab, direction encoding or
+//               time slab), in this order in every build: the order of the fp32 sums is part of the results.
 #include "nm_internal.cuh"
 #include "nm_pe.cuh"
 #include "tc_common.cuh"
@@ -68,19 +72,26 @@ __host__ __device__ constexpr int tc_slabs_per_tile(bool v = true, bool t = fals
 }
 static_assert(tc_slabs_per_tile(true, true) <= TC_MAX_SLABS && tc_slabs_per_tile(true) <= TC_MAX_SLABS, "slab table too small");
 
+// Shared memory.  The render kernels keep activations in registers only and have no activation blocks, which the
+// training forward keeps as the source of its stash stores.  Ring depth: 4 slots, measured 1-2 % faster than 6 in
+// k_mlp_tc<false>; 6 in the view-independent render kernel, which spills 32 B with 4 (DESIGN.md §4).
+template <bool kTrain, bool kView>
 struct TcCfg {
   static constexpr int THREADS = 256;                  // two consumer warpgroups
-  // per warpgroup: act[4 k-blocks] | position encoding | direction encoding
-  static constexpr int OFF_POS = 4 * TC_KB_BYTES;
-  static constexpr int OFF_DIR = 5 * TC_KB_BYTES;
-  static constexpr int WG_BYTES = 6 * TC_KB_BYTES;
+  static constexpr int NSLOT = kTrain || kView ? 4 : 6;   // depth of the weight ring
+  // per warpgroup: [act[4 k-blocks], kTrain only] | position encoding | direction encoding
+  static constexpr int OFF_POS = kTrain ? 4 * TC_KB_BYTES : 0;
+  static constexpr int OFF_DIR = OFF_POS + TC_KB_BYTES;
+  static constexpr int WG_BYTES = OFF_DIR + TC_KB_BYTES;
   static constexpr int OFF_RING = 2 * WG_BYTES;
-  static constexpr int OFF_BAR = OFF_RING + TC_NSLOT * TC_SLAB_BYTES;
-  static constexpr int OFF_CONST = OFF_BAR + 16 * TC_NSLOT;         // the constant table (k_tc_consts), fp32
+  static constexpr int OFF_BAR = OFF_RING + NSLOT * TC_SLAB_BYTES;  // full barriers (8 B), then release counters (4 B)
+  static constexpr int OFF_CONST = OFF_BAR + 16 * NSLOT;            // the constant table (k_tc_consts), fp32
   static constexpr int SMEM_USED = OFF_CONST + 4 * TC_CONST_FLOATS;
   static constexpr int SMEM_BYTES = SMEM_USED + 1024;               // + alignment slack of the 1024-byte swizzle atoms
 };
-static_assert(TcCfg::SMEM_BYTES <= 232448, "shared memory of the forward kernel exceeds 227 KB");
+static_assert(TcCfg<false, false>::SMEM_BYTES <= 232448 && TcCfg<false, true>::SMEM_BYTES <= 232448 &&
+              TcCfg<true, false>::SMEM_BYTES <= 232448 && TcCfg<true, true>::SMEM_BYTES <= 232448,
+              "shared memory of the forward kernel exceeds 227 KB");
 
 // constant table of the epilogue: [0, 256) alpha_linear.weight | 256..258 rgb bias | 259 alpha bias
 // (view-independent nets: [0, 256) unused | 256..259 output_linear.bias)
@@ -211,14 +222,16 @@ __device__ __forceinline__ void track_range(uint32_t& rng, uint32_t packed) {
 
 // ---------------------------------------------------------------------------------------------
 // Epilogue of NC accumulator columns of this thread's two rows rA, rA + 8 (columns 8j + 2q, +1: tc_common.cuh):
-// the alpha head on step 7 (fp32 FFMAs on the ReLU of the unrounded accumulators), ReLU, saturating f16x2 pack,
-// swizzled 4-byte stores into the activation block that is the next step's A operand, and the ReLU sign words
+// the alpha head on step 7 (fp32 FFMAs on the ReLU of the unrounded accumulators), ReLU, saturating f16x2 pack into
+// the next step's A operand: `a`, its register fragments (a[2j] / a[2j + 1]: rows rA / rA + 8 of columns 8j + 2q, +1;
+// K slice k of the next step reads a[4k..4k+3]), or with SMEM swizzled 4-byte stores into the activation block, and the ReLU sign words
 // (word w = columns 32w..32w+31; bits 0-7 / 8-15: even / odd columns of the first 16, bits 16-31 the same for the
 // next 16) as this thread's share, OR-reduced over the quad afterwards.
 // ---------------------------------------------------------------------------------------------
-template <int NC, bool RELU, bool ALPHA, bool SIGNS>
-__device__ __forceinline__ void fwd_epi(const float (&d)[128], uint8_t* act, int rA, int q, const float* s_walpha,
-                                        float (&alpha)[2], uint32_t (&wA)[8], uint32_t (&wB)[8], bool track, uint32_t& rng) {
+template <int NC, bool RELU, bool ALPHA, bool SIGNS, bool SMEM>
+__device__ __forceinline__ void fwd_epi(const float (&d)[128], uint32_t (&a)[64], uint8_t* act, int rA, int q,
+                                        const float* s_walpha, float (&alpha)[2], uint32_t (&wA)[8], uint32_t (&wB)[8],
+                                        bool track, uint32_t& rng) {
   const int rB = rA + 8;
 #pragma unroll
   for (int j = 0; j < NC / 8; ++j) {
@@ -230,9 +243,14 @@ __device__ __forceinline__ void fwd_epi(const float (&d)[128], uint8_t* act, int
       alpha[1] = fmaf(fmaxf(y0, 0.f), w.x, fmaf(fmaxf(y1, 0.f), w.y, alpha[1]));
     }
     const uint32_t pA = pack2<RELU>(x0, x1), pB = pack2<RELU>(y0, y1);
-    uint8_t* blk = act + (j >> 3) * TC_KB_BYTES;
-    *reinterpret_cast<uint32_t*>(blk + swz_off(rA, c)) = pA;
-    *reinterpret_cast<uint32_t*>(blk + swz_off(rB, c)) = pB;
+    if (SMEM) {
+      uint8_t* blk = act + (j >> 3) * TC_KB_BYTES;
+      *reinterpret_cast<uint32_t*>(blk + swz_off(rA, c)) = pA;
+      *reinterpret_cast<uint32_t*>(blk + swz_off(rB, c)) = pB;
+    } else {
+      a[2 * j] = pA;
+      a[2 * j + 1] = pB;
+    }
     if (track) { track_range<RELU>(rng, pA); track_range<RELU>(rng, pB); }
     if (SIGNS) {
       const __half2 zero2 = __float2half2_rn(0.f);
@@ -260,7 +278,7 @@ __device__ __forceinline__ void quad_or(uint32_t (&w)[8]) {
 template <bool kTrain, bool kView, bool kTime = false>
 __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
   static_assert(!kTime || kView, "NeRF-T nets are view-dependent");
-  using C = TcCfg;
+  using C = TcCfg<kTrain, kView>;
   constexpr int SLABS = tc_slabs_per_tile(kView, kTime);
   constexpr int STEPS = tc_steps(kView);
   constexpr int LAST = STEPS - 1;                       // the output step: rgb (N = 16) or output_linear (N = 16)
@@ -274,39 +292,40 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
   uint8_t* wbuf = smem + wg * C::WG_BYTES;
   const uint32_t wbase = sbase + wg * C::WG_BYTES;
   float* s_const = reinterpret_cast<float*>(smem + C::OFF_CONST);
-  const TcRing R{sbase + C::OFF_RING, sbase + C::OFF_BAR};
+  const TcRing<C::NSLOT> R{sbase + C::OFF_RING, sbase + C::OFF_BAR};
 
   for (int i = threadIdx.x; i < TC_CONST_FLOATS; i += C::THREADS) s_const[i] = __ldg(P.consts + i);
   const long long my_tiles = blockIdx.x < P.n_tiles ? (P.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
   const uint32_t total = (uint32_t)(my_tiles * SLABS);
-  // Refills: the warpgroup that releases a slot second issues the slab TC_NSLOT places further on, right away.  A
+  // Refills: the warpgroup that releases a slot second issues the slab NSLOT places further on, right away.  A
   // per-slot release counter in place of an `empty` barrier decides which one that is, so neither warpgroup ever waits
   // for the other's release: warpgroup 0 keeps issuing MMAs on the slabs already in the ring while warpgroup 1 is behind
   // (e.g. in its epilogue), and the other way round.
-  const uint32_t rel = sbase + C::OFF_BAR + 8 * TC_NSLOT;          // TC_NSLOT release counters (u32)
+  const uint32_t rel = sbase + C::OFF_BAR + 8 * C::NSLOT;          // NSLOT release counters (u32)
   auto refill = [&](uint32_t qq) {
     const uint32_t j = qq % SLABS, off = P.plan.lin_off[j], bytes = P.plan.lin_off[j + 1] - off;
     mbar_arrive_expect_tx(R.full(qq), bytes);
     bulk_g2s(R.slot(qq), P.wimg + off, bytes, R.full(qq));
   };
   if (threadIdx.x == 0) {
-    for (int i = 0; i < TC_NSLOT; ++i) {
+    for (int i = 0; i < C::NSLOT; ++i) {
       mbar_init(R.full(i), 1);
       st_shared_u32(rel + 4 * i, 0);
     }
     fence_mbar_init();
-    for (uint32_t i = 0; i < TC_NSLOT && i < total; ++i) refill(i);
+    for (uint32_t i = 0; i < C::NSLOT && i < total; ++i) refill(i);
   }
   __syncthreads();
   auto release = [&](uint32_t qq) {
     // acq_rel: the first releaser's finished MMA reads of the slot are ordered before the second one's refill
-    if (wtid == 0 && qq + TC_NSLOT < total && (atom_add_acq_rel_cta(rel + 4 * (qq % TC_NSLOT), 1) & 1)) refill(qq + TC_NSLOT);
+    if (wtid == 0 && qq + C::NSLOT < total && (atom_add_acq_rel_cta(rel + 4 * (qq % C::NSLOT), 1) & 1)) refill(qq + C::NSLOT);
     __syncwarp();
   };
 
   const float4 ob = *reinterpret_cast<const float4*>(s_const + TC_CONST_OUT);
   float d[128];
   float d16[8];
+  uint32_t a[64];                                       // the previous step's output: A fragments of 16 K slices
   uint32_t rng = 0;
   uint32_t qbase = 0;
   const long long rperiod = my_tiles < 64 ? my_tiles : 64;
@@ -334,6 +353,10 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
         nm_fetch_sample_at<kTime ? 4 : 3>(P.in, row0 + r, g, p, v);
         if (kTime) t = nm_fetch_time(P.in, row0 + r);
       }
+      // rendering: the previous tile's last MMAs on the encoding blocks (the bias slab of step 8 / 7, the direction
+      // k-block of step 9) must have retired in all four warps before the blocks are overwritten (in the training
+      // forward the barrier before the epilogue of step 9 / 7 orders them)
+      if (!kTrain && it > 0) wg_sync(wg);
       uint32_t e[32];
       if (wtid < 64) {
         encode_f16(P.pos_pe, p, e, 30);
@@ -349,30 +372,89 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
       wg_sync(wg);
     }
     float alpha[2] = {0.f, 0.f};
+    // rendering: unrolled, so each step's k-blocks and epilogue touch a fixed part of `a` and only that part is live
+#pragma unroll (kTrain ? 1 : STEPS)
     for (int s = 0; s < STEPS; ++s) {
       const int nkb = step_nkb(s, kView, kTime);
       wgmma_fence();
-      for (int kb = 0; kb < nkb; ++kb) {
-        const uint32_t qq = qbase + kb;
-        R.wait_full(qq);
-        const bool time = kb_is_time(s, kb, kTime);
-        const uint32_t a_addr = kb_is_pos(s, kb, kView, kTime) ? wbase + C::OFF_POS
-                              : (kb_is_dir(s, kb, kView) || time) ? wbase + C::OFF_DIR
-                                                 : wbase + kb_act_index(s, kb) * TC_KB_BYTES;
-        // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
-        // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab), a time
-        // slab two on K slices 2..3 (channels 32..63 of the direction block)
-        const bool bias = kb_is_bias(s, kb, kView);
-        const int k0 = bias ? 3 : (time ? 2 : 0), k1 = kb_is_dir(s, kb, kView) ? 2 : 4;
-        const uint64_t a_desc = gmma_desc_k(a_addr), b_desc = gmma_desc_k(R.slot(qq));
-        for (int k = k0; k < k1; ++k) {
-          const uint32_t acc = (kb | (k - k0)) != 0;
-          if (s <= (kView ? 8 : 7)) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
-          else if (kView && s == 9) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
-          else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
+      if constexpr (kTrain) {
+        // training forward: every k-block's A operand from shared memory (the activation blocks are the stash's source;
+        // holding `a` as well makes these kernels spill)
+        for (int kb = 0; kb < nkb; ++kb) {
+          const uint32_t qq = qbase + kb;
+          R.wait_full(qq);
+          const bool time = kb_is_time(s, kb, kTime);
+          const uint32_t a_addr = kb_is_pos(s, kb, kView, kTime) ? wbase + C::OFF_POS
+                                : (kb_is_dir(s, kb, kView) || time) ? wbase + C::OFF_DIR
+                                                   : wbase + kb_act_index(s, kb) * TC_KB_BYTES;
+          // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
+          // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab), a time
+          // slab two on K slices 2..3 (channels 32..63 of the direction block)
+          const bool bias = kb_is_bias(s, kb, kView);
+          const int k0 = bias ? 3 : (time ? 2 : 0), k1 = kb_is_dir(s, kb, kView) ? 2 : 4;
+          const uint64_t a_desc = gmma_desc_k(a_addr), b_desc = gmma_desc_k(R.slot(qq));
+          for (int k = k0; k < k1; ++k) {
+            const uint32_t acc = (kb | (k - k0)) != 0;
+            if (s <= (kView ? 8 : 7)) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+            else if (kView && s == 9) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+            else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
+          }
+          wgmma_commit();
+          if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
         }
-        wgmma_commit();
-        if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
+      } else {
+        const bool wide = s <= (kView ? 8 : 7), views = kView && s == 9;     // N = 256 / 128 (views) / 16 (output)
+        int kb = 0;
+        // one k-block: wait for its slab, issue its MMAs (`issue(b_desc, first k-block of the step)`), commit, and
+        // release the previous k-block's slab once its MMAs have retired
+        auto kblock = [&](auto&& issue) {
+          const uint32_t qq = qbase + kb;
+          R.wait_full(qq);
+          issue(gmma_desc_k(R.slot(qq)), kb == 0);
+          wgmma_commit();
+          if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
+          ++kb;
+        };
+        // a k-block whose A operand is an encoding block in shared memory, K slices k0..k1-1.  K advances by 32 B (= 2
+        // in descriptor address units) inside the 128-byte swizzle atom.
+        auto smem_kblock = [&](uint32_t a_addr, int k0, int k1) {
+          kblock([&](uint64_t b_desc, bool first) {
+            const uint64_t a_desc = gmma_desc_k(a_addr);
+            for (int k = k0; k < k1; ++k) {
+              const uint32_t acc = !first || k > k0;
+              if (wide) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+              else if (views) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+              else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
+            }
+          });
+        };
+        if (s == 0 || s == 5) smem_kblock(wbase + C::OFF_POS, 0, 4);       // position encoding (step 5: "input first", :131)
+        if (s > 0) {
+          const int nact = kView && s == LAST ? 2 : 4;                      // rgb reads the 128 columns of the views layer
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            if (j < nact) {
+              kblock([&](uint64_t b_desc, bool first) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                  const uint32_t* f = a + 16 * j + 4 * k;
+                  const uint32_t acc = !first || k > 0;
+                  if (wide) wgmma_n256_rs(d, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
+                  else if (views) wgmma_n128_rs(d, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
+                  else wgmma_n16_rs(d16, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
+                }
+              });
+            }
+          }
+        }
+        // the trailing k-block: a bias slab is one K = 16 MMA on the last K slice (channels 48..63 of the position
+        // encoding x columns 48..63 of the slab), the direction encoding two on K slices 0..1, a time slab two on K
+        // slices 2..3 (channels 32..63 of the direction block)
+        if (kb < nkb) {
+          if (kb_is_bias(s, kb, kView)) smem_kblock(wbase + C::OFF_POS, 3, 4);
+          else if (kb_is_dir(s, kb, kView)) smem_kblock(wbase + C::OFF_DIR, 0, 2);
+          else smem_kblock(wbase + C::OFF_DIR, 2, 4);
+        }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(d);
@@ -380,19 +462,21 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
       release(qbase + nkb - 1);
       qbase += nkb;
       if (s < LAST) {
-        // the MMAs of this step read the activation buffer, the stash stores of the previous step still may: both must
-        // be done before the epilogue overwrites it
-        if (kTrain && wtid == 0) tma_store_wait_read();
-        wg_sync(wg);
+        // training forward: the MMAs of this step read the activation blocks, the stash stores of the previous step
+        // still may: both must be done before the epilogue overwrites them
+        if (kTrain) {
+          if (wtid == 0) tma_store_wait_read();
+          wg_sync(wg);
+        }
         uint32_t wA[8] = {0, 0, 0, 0, 0, 0, 0, 0}, wB[8] = {0, 0, 0, 0, 0, 0, 0, 0};
         const float* s_walpha = s_const + TC_CONST_ALPHA;
-        if (s == 7) fwd_epi<256, true, kView, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
-        else if (kView && s == 8) fwd_epi<256, false, false, false>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
-        else if (s == 9) fwd_epi<128, true, false, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
-        else fwd_epi<256, true, false, kTrain>(d, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
-        fence_async_smem();
-        wg_sync(wg);
+        if (s == 7) fwd_epi<256, true, kView, kTrain, kTrain>(d, a, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else if (kView && s == 8) fwd_epi<256, false, false, false, kTrain>(d, a, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else if (s == 9) fwd_epi<128, true, false, kTrain, kTrain>(d, a, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
+        else fwd_epi<256, true, false, kTrain, kTrain>(d, a, wbuf, rA, q, s_walpha, alpha, wA, wB, track, rng);
         if (kTrain) {
+          fence_async_smem();
+          wg_sync(wg);
           if (wtid == 0) {
             if (!kView || s < 8) tma_store_rows(&P.map_x, wbase, 0, 4, row0, s);
             else if (s == 8) tma_store_rows(&P.map_f, wbase, 0, 4, row0, 0);
@@ -446,17 +530,17 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
 
 // view-dependent nets (use_viewdirs=True): render (kTrain = false) and training forward
 template <bool kTrain>
-__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
+__global__ void __launch_bounds__(TcCfg<kTrain, true>::THREADS, 1) k_mlp_tc(const __grid_constant__ TcParams P) {
   mlp_tc_body<kTrain, true>(P);
 }
 // view-independent nets (use_viewdirs=False): no direction input, output_linear head
 template <bool kTrain>
-__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc_noview(const __grid_constant__ TcParams P) {
+__global__ void __launch_bounds__(TcCfg<kTrain, false>::THREADS, 1) k_mlp_tc_noview(const __grid_constant__ TcParams P) {
   mlp_tc_body<kTrain, false>(P);
 }
 // NeRF-T nets (view-dependent, position input (x, y, z, t)): render (kTrain = false) and training forward
 template <bool kTrain>
-__global__ void __launch_bounds__(TcCfg::THREADS, 1) k_mlp_tc_nerft(const __grid_constant__ TcParams P) {
+__global__ void __launch_bounds__(TcCfg<kTrain, true>::THREADS, 1) k_mlp_tc_nerft(const __grid_constant__ TcParams P) {
   mlp_tc_body<kTrain, true, true>(P);
 }
 
@@ -667,10 +751,11 @@ static int launch_tc(nm_ctx* ctx, const TcParams& P, cudaStream_t st) {
   void (*kernel)(const TcParams);
   if constexpr (kTime) kernel = k_mlp_tc_nerft<kTrain>;
   else kernel = kView ? k_mlp_tc<kTrain> : k_mlp_tc_noview<kTrain>;
-  NM_SET_SMEM_ONCE(ctx, kernel, TcCfg::SMEM_BYTES);
+  using C = TcCfg<kTrain, kView>;
+  NM_SET_SMEM_ONCE(ctx, kernel, C::SMEM_BYTES);
   long long ctas = ctx->sm_count;
   if (P.n_tiles < ctas) ctas = P.n_tiles > 0 ? P.n_tiles : 1;
-  kernel<<<(unsigned)ctas, TcCfg::THREADS, TcCfg::SMEM_BYTES, st>>>(P);
+  kernel<<<(unsigned)ctas, C::THREADS, C::SMEM_BYTES, st>>>(P);
   NM_CHECK_LAUNCH(ctx);
   return NM_OK;
 }

@@ -30,10 +30,11 @@ __host__ __device__ constexpr int bw_const_floats(bool view) { return view ? 256
 template <bool kView>
 struct BwCfg {
   static constexpr int THREADS = 256;                      // two consumer warpgroups
+  static constexpr int NSLOT = 4;                           // depth of the weight ring
   static constexpr int WG_BYTES = 4 * TC_KB_BYTES;          // per warpgroup: act[4 k-blocks]
   static constexpr int OFF_RING = 2 * WG_BYTES;
-  static constexpr int OFF_BAR = OFF_RING + TC_NSLOT * TC_SLAB_BYTES;
-  static constexpr int OFF_CONST = OFF_BAR + 16 * TC_NSLOT;  // w_alpha[256] | w_rgb[3][128] (or w_out[4][256]), fp32
+  static constexpr int OFF_BAR = OFF_RING + NSLOT * TC_SLAB_BYTES;
+  static constexpr int OFF_CONST = OFF_BAR + 16 * NSLOT;     // w_alpha[256] | w_rgb[3][128] (or w_out[4][256]), fp32
   static constexpr int SMEM_USED = OFF_CONST + 4 * bw_const_floats(kView);
   static constexpr int SMEM_BYTES = SMEM_USED + 1024;
 };
@@ -126,7 +127,7 @@ __device__ __forceinline__ void mlp_tc_bwd_body(const BwParams& P) {
   const uint32_t abase = sbase + wg * C::WG_BYTES;
   float* s_walpha = reinterpret_cast<float*>(smem + C::OFF_CONST);
   float* s_wrgb = s_walpha + 256;
-  const TcRing R{sbase + C::OFF_RING, sbase + C::OFF_BAR};
+  const TcRing<C::NSLOT> R{sbase + C::OFF_RING, sbase + C::OFF_BAR};
 
   if (kView) {
     s_walpha[threadIdx.x] = __ldg(P.w_alpha + threadIdx.x);
@@ -139,14 +140,14 @@ __device__ __forceinline__ void mlp_tc_bwd_body(const BwParams& P) {
   uint32_t pq = 0;                                   // producer (thread 0): next slab to issue
   auto produce = [&]() {
     if (pq >= total) return;
-    if (pq >= TC_NSLOT) mbar_wait(R.empty(pq), (pq / TC_NSLOT - 1) & 1);
+    if (pq >= C::NSLOT) mbar_wait(R.empty(pq), (pq / C::NSLOT - 1) & 1);
     mbar_arrive_expect_tx(R.full(pq), TC_SLAB_BYTES);
     bulk_g2s(R.slot(pq), P.wimg + (size_t)(pq % SLABS) * TC_SLAB_BYTES, TC_SLAB_BYTES, R.full(pq));
     ++pq;
   };
   if (threadIdx.x == 0) {
     R.init();
-    for (int i = 0; i < TC_NSLOT; ++i) produce();
+    for (int i = 0; i < C::NSLOT; ++i) produce();
   }
   __syncthreads();
   auto release = [&](uint32_t qq) {

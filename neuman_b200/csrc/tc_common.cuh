@@ -8,7 +8,6 @@
 #define TC_WG_ROWS 64              // sample rows per consumer warpgroup (wgmma M = 64)
 #define TC_KB_BYTES (TC_WG_ROWS * 128)   // one A k-block of a warpgroup: 64 rows x 128 B
 #define TC_SLAB_BYTES 32768        // one weight k-block: 256 rows x 128 B
-#define TC_NSLOT 4                 // depth of the weight ring
 
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -125,6 +124,40 @@ __device__ __forceinline__ void wgmma_n16_mn(float (&d)[8], uint64_t a_desc, uin
       : "l"(a_desc), "l"(b_desc), "r"(accum));
 }
 
+// The same with A from registers: {a0..a3} = the f16x2 A fragment of the thread's rows rA, rA + 8 (a0 / a1: columns
+// 2q, 2q + 1 of rows rA / rA + 8, a2 / a3: columns 2q + 8, 2q + 9).  It is the layout of accumulator columns 16k..16k+15
+// (d[8k..8k+7] above, packed pairwise), so one MMA's output feeds the next one's A operand without shared memory.
+__device__ __forceinline__ void wgmma_n256_rs(float (&d)[128], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
+                                              uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "{%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_n128_rs(float (&d)[128], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
+                                              uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_n16_rs(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
+                                             uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "{%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(accum));
+}
+
 // {lo, hi} -> packed f16x2 (lo in the low half), optional ReLU
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi, bool relu) {
   uint32_t d;
@@ -189,18 +222,19 @@ __device__ __forceinline__ void tma_store_rows(const CUtensorMap* map, uint32_t 
   tma_store_commit();
 }
 
-// One warpgroup's view of the weight ring: the slabs of a launch are consumed in a fixed order by both warpgroups; a slab's
-// slot is refilled once both have released it.  In the backward chain thread 0 of the CTA is the producer: it issues the
-// first TC_NSLOT slabs and, after each of its own releases, waits on `empty` and issues the slab TC_NSLOT places further
-// on.  The forward kernel (mlp_tc.cu) uses the slots and `full` barriers only: there the second releaser refills.
+// One warpgroup's view of an NSLOT-deep weight ring: the slabs of a launch are consumed in a fixed order by both warpgroups;
+// a slab's slot is refilled once both have released it.  In the backward chain thread 0 of the CTA is the producer: it issues
+// the first NSLOT slabs and, after each of its own releases, waits on `empty` and issues the slab NSLOT places further on.
+// The forward kernel (mlp_tc.cu) uses the slots and `full` barriers only: there the second releaser refills.
+template <int NSLOT>
 struct TcRing {
-  uint32_t ring, bar;       // shared addresses: TC_NSLOT slots of TC_SLAB_BYTES; full[TC_NSLOT] then empty[TC_NSLOT]
-  __device__ uint32_t slot(uint32_t q) const { return ring + (q % TC_NSLOT) * TC_SLAB_BYTES; }
-  __device__ uint32_t full(uint32_t q) const { return bar + 8 * (q % TC_NSLOT); }
-  __device__ uint32_t empty(uint32_t q) const { return bar + 8 * (TC_NSLOT + q % TC_NSLOT); }
-  __device__ void wait_full(uint32_t q) const { mbar_wait(full(q), (q / TC_NSLOT) & 1); }
+  uint32_t ring, bar;       // shared addresses: NSLOT slots of TC_SLAB_BYTES; full[NSLOT] then empty[NSLOT]
+  __device__ uint32_t slot(uint32_t q) const { return ring + (q % NSLOT) * TC_SLAB_BYTES; }
+  __device__ uint32_t full(uint32_t q) const { return bar + 8 * (q % NSLOT); }
+  __device__ uint32_t empty(uint32_t q) const { return bar + 8 * (NSLOT + q % NSLOT); }
+  __device__ void wait_full(uint32_t q) const { mbar_wait(full(q), (q / NSLOT) & 1); }
   __device__ void init() const {
-    for (int i = 0; i < TC_NSLOT; ++i) { mbar_init(bar + 8 * i, 1); mbar_init(bar + 8 * (TC_NSLOT + i), 2); }
+    for (int i = 0; i < NSLOT; ++i) { mbar_init(bar + 8 * i, 1); mbar_init(bar + 8 * (NSLOT + i), 2); }
     fence_mbar_init();
   }
 };

@@ -3,8 +3,10 @@
     python tools/fwd_digest.py dump OUT.json [--root TREE]     # run TREE's library (default: this tree) on seeded inputs
     python tools/fwd_digest.py compare A.json B.json           # exit 1 unless every record is identical
 
-`dump` runs k_mlp_tc on seeded inputs and records a SHA-256 of every output buffer: the training forward's raw, activation
-stash (st_x, st_f, st_v) and sign words, and the inference raw in per-sample, per-ray-view and fused ray modes.  Sizes
+`dump` runs the tensor-core forward on seeded inputs and records a SHA-256 of every output buffer: the training forward's raw,
+activation stash (st_x, st_f, st_v) and sign words, and the inference raw in per-sample, per-ray-view and fused ray modes,
+for view-dependent nets (posenc and rotate), a view-independent net (no st_f / st_v, 8 sign-word planes) and a NeRF-T net
+([n,4] points; no fused ray mode, which NeRF-T slots do not take).  Sizes
 cover ragged tiles, several waves of the persistent grid and a frame-sized ray chunk.  Its frames section renders with
 every driver (vanilla coarse-only and coarse + fine, smpl_nerf canonical and posed, hybrid, multi-person with 2 and 3
 actors), each with host and device output, a pixel range and a pixel list, the default chunk and a ragged one, and
@@ -33,28 +35,35 @@ def dump(out, root):
     torch.cuda.set_device(dev)
     coarse, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False), 1)
     human, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False, posenc="rotate"), 2)
+    noview, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False, use_viewdirs=False), 3)
+    nerft, _ = scenes.seed_nets(nb.build_nerf, nb.default_opt(use_cuda=False, raw_pos_dim=4), 4)
     T = 128 * torch.cuda.get_device_properties(0).multi_processor_count
     res = {"lib": _lib.LIB_PATH}
-    for name, j in (("coarse", coarse.to(dev)), ("human", human.to(dev))):
+    for name, j in (("coarse", coarse.to(dev)), ("human", human.to(dev)), ("noview", noview.to(dev)), ("nerft", nerft.to(dev))):
+        view, time = name != "noview", name == "nerft"
         ctx = ops._ctx_for(torch.empty(1, device=dev))
         slot = ops.net_slot(j, ctx)
         for n in (1, 129, 4173, 3 * T - 5):
             g = torch.Generator(device=dev).manual_seed(n)
             pts = torch.randn(n, 3, device=dev, generator=g) * 1.5
             views = torch.nn.functional.normalize(torch.randn(n, 3, device=dev, generator=g), dim=-1)
+            if time:                                 # (x, y, z, t), t in [0, 1)
+                pts = torch.cat([pts, torch.rand(n, 1, device=dev, generator=g)], dim=1).contiguous()
             # training forward, per-sample views
             raw = torch.empty(n, 4, device=dev)
             sx = torch.empty(8, n, 256, device=dev, dtype=torch.float16)
             sf = torch.empty(n, 256, device=dev, dtype=torch.float16)
             sv = torch.empty(n, 128, device=dev, dtype=torch.float16)
-            sm = torch.empty(9, n, 8, device=dev, dtype=torch.int32)
+            sm = torch.empty(9 if view else 8, n, 8, device=dev, dtype=torch.int32)
             ctx.check(ctx.lib.nm_mlp_forward_train(ctx.h, slot, _p(pts), _p(views), n, 0, _p(raw), _p(sx), _p(sf), _p(sv),
                                                    _p(sm), ctx.stream()))
             torch.cuda.synchronize()
-            for k, v in (("raw", raw), ("st_x", sx), ("st_f", sf), ("st_v", sv), ("st_m", sm)):
+            outs = (("raw", raw), ("st_x", sx), ("st_f", sf), ("st_v", sv), ("st_m", sm)) if view else \
+                (("raw", raw), ("st_x", sx), ("st_m", sm))
+            for k, v in outs:
                 res[f"{name}/train/n={n}/{k}"] = _digest(v)
             # inference, per-sample views and one view row per 7 samples (n rounded down to a multiple of 7)
-            for group in (0, 7):
+            for group in (0,) if time else (0, 7):
                 m = n if group == 0 else n - n % group
                 if m == 0:
                     continue
@@ -65,7 +74,7 @@ def dump(out, root):
                 torch.cuda.synchronize()
                 res[f"{name}/infer/n={m}/group={group}/raw"] = _digest(raw)
         # fused ray mode (pts = o + d z), up to a frame's chunk of 32768 rays x 256 samples
-        for R, S in ((1, 1), (33, 33), (97, 128), (4096, 128), (32768, 256)):
+        for R, S in () if time else ((1, 1), (33, 33), (97, 128), (4096, 128), (32768, 256)):
             g = torch.Generator(device=dev).manual_seed(R * 1000 + S)
             o = torch.randn(R, 3, device=dev, generator=g) * 0.3
             d = torch.nn.functional.normalize(torch.randn(R, 3, device=dev, generator=g), dim=-1)
