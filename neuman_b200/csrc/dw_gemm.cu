@@ -62,44 +62,33 @@ __global__ void __launch_bounds__(DW_THREADS, 1) k_dw_gemm(const __grid_constant
   const int lane = threadIdx.x & 31, q = lane & 3;
   const int half = blockIdx.x & 1;                   // output channels [128 half, 128 half + 128) of the work item
   const int item = blockIdx.x >> 1;
-  auto bar_full = [&](int i) { return sbase + C::OFF_BAR + 8 * i; };
-  auto bar_empty = [&](int i) { return sbase + C::OFF_BAR + 8 * (DW_STAGES + i); };
+  const TcRing<DW_STAGES, DW_STAGE_BYTES> R{sbase + C::OFF_STAGE, sbase + C::OFF_BAR};
 
   const DwWork W = P.work[item < P.n_work ? item : 0];
   const bool has_work = item < P.n_work && 128 * half < W.m_rows;
-  const int n_stages = has_work ? (int)((W.row1 - W.row0 + DW_ROWS - 1) / DW_ROWS) : 0;
+  const uint32_t n_stages = has_work ? (uint32_t)((W.row1 - W.row0 + DW_ROWS - 1) / DW_ROWS) : 0;
 
   for (int i = threadIdx.x; i < DW_BOX_BYTES / 4; i += DW_THREADS)
     reinterpret_cast<uint32_t*>(smem + C::OFF_ONES)[i] = 0x3C003C00u;      // fp16 {1.0, 1.0}
   fence_async_smem();                                                      // generic-proxy writes -> tensor-core reads
-  int prod = 0;                                                            // producer (thread 0): next stage to load
-  auto produce = [&]() {
-    if (prod >= n_stages) return;
-    const int slot = prod % DW_STAGES, gen = prod / DW_STAGES;
-    if (gen > 0) mbar_wait(bar_empty(slot), (gen - 1) & 1);
-    mbar_arrive_expect_tx(bar_full(slot), DW_STAGE_BYTES);
-    const uint32_t dst = sbase + C::OFF_STAGE + slot * DW_STAGE_BYTES;
-    const int row = (int)(W.row0 + (long long)prod * DW_ROWS);
+  auto fill = [&](uint32_t st) {                                           // stage st: rows row0 + 64 st ..
+    mbar_arrive_expect_tx(R.full(st), DW_STAGE_BYTES);
+    const uint32_t dst = R.slot(st);
+    const int row = (int)(W.row0 + (long long)st * DW_ROWS);
     const CUtensorMap* ma = &P.maps[W.a_map];
     const CUtensorMap* mb = &P.maps[W.b_map];
-    for (int b = 0; b < 2; ++b) tma_load_3d(dst + b * DW_BOX_BYTES, ma, 128 * half + 64 * b, row, W.a_plane, bar_full(slot));
-    for (int b = 0; b < 4; ++b) tma_load_3d(dst + (2 + b) * DW_BOX_BYTES, mb, 64 * b, row, W.b_plane, bar_full(slot));
-    ++prod;
+    for (int b = 0; b < 2; ++b) tma_load_3d(dst + b * DW_BOX_BYTES, ma, 128 * half + 64 * b, row, W.a_plane, R.full(st));
+    for (int b = 0; b < 4; ++b) tma_load_3d(dst + (2 + b) * DW_BOX_BYTES, mb, 64 * b, row, W.b_plane, R.full(st));
   };
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < DW_STAGES; ++i) { mbar_init(bar_full(i), 1); mbar_init(bar_empty(i), 2); }
-    fence_mbar_init();
-    for (int i = 0; i < DW_STAGES; ++i) produce();
-  }
+  if (threadIdx.x == 0) R.init(n_stages, fill);
   __syncthreads();
   if (n_stages == 0) return;
 
   float d[128], db[8];
   const uint64_t ones_desc = gmma_desc_mn(sbase + C::OFF_ONES, DW_BOX_BYTES);
-  for (int st = 0; st < n_stages; ++st) {
-    const int slot = st % DW_STAGES;
-    mbar_wait(bar_full(slot), (st / DW_STAGES) & 1);
-    const uint32_t base = sbase + C::OFF_STAGE + slot * DW_STAGE_BYTES;
+  for (uint32_t st = 0; st < n_stages; ++st) {
+    R.wait_full(st);
+    const uint32_t base = R.slot(st);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < DW_ROWS / 16; ++kk) {       // 16 K rows = two 8-row groups = 2048 B
@@ -109,12 +98,7 @@ __global__ void __launch_bounds__(DW_THREADS, 1) k_dw_gemm(const __grid_constant
       wgmma_n16_mn(db, a_desc, ones_desc, (st | kk) != 0);
     }
     wgmma_commit();
-    if (st > 0) {
-      wgmma_wait<1>();
-      if (wtid == 0) mbar_arrive_local(bar_empty((st - 1) % DW_STAGES));
-      if (threadIdx.x == 0) produce();
-      __syncwarp();
-    }
+    if (st > 0) { wgmma_wait<1>(); R.release(st - 1, n_stages, fill); }
   }
   wgmma_wait<0>();
   wgmma_fence_regs(d);

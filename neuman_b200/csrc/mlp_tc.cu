@@ -18,10 +18,11 @@
 //               TcCfg::NSLOT-deep ring (tc_common.cuh: TcRing): 4 slots, 6 in the view-independent render kernel.
 //   epilogue  : accumulator registers -> ReLU -> cvt to f16x2 -> `a`, the A register fragments of the next step's
 //               MMAs (the accumulator layout of 16 columns is the A fragment layout of one K = 16 slice).  The
-//               training forward also writes the swizzled activation block in shared memory, the source of the
-//               stash's TMA stores.  A step's k-blocks: the position encoding from shared memory (steps 0 and 5),
-//               the activation k-blocks from `a`, then one from shared memory (bias slab, direction encoding or
-//               time slab), in this order in every build: the order of the fp32 sums is part of the results.
+//               training forward writes the swizzled activation block in shared memory instead, the source of the
+//               stash's TMA stores.  One step loop for both: a step's k-blocks are the position encoding from shared
+//               memory (steps 0 and 5), the activation k-blocks (from `a`, or in training from the activation block),
+//               then one from shared memory (bias slab, direction encoding or time slab), in this order in every
+//               kernel: the order of the fp32 sums is part of the results.
 #include "nm_internal.cuh"
 #include "nm_pe.cuh"
 #include "tc_common.cuh"
@@ -59,12 +60,8 @@ __host__ __device__ constexpr bool kb_is_bias(int s, int kb, bool v = true) {
 }
 __host__ __device__ constexpr bool kb_is_time(int s, int kb, bool t) { return t && ((s == 0 && kb == 1) || (s == 5 && kb == 5)); }
 __host__ __device__ constexpr int step_N(int s, bool v = true) { return s <= 7 || (v && s == 8) ? 256 : (v && s == 9 ? 128 : 16); }
-// k-block kb of step s reads the position encoding / the direction encoding (else activation block `act_kb`)
-__host__ __device__ constexpr bool kb_is_pos(int s, int kb, bool v = true, bool t = false) {
-  return (s == 0 && (!t || kb == 0)) || (s == 5 && kb == 0) || kb_is_bias(s, kb, v);
-}
+// k-block kb of step s reads the direction encoding
 __host__ __device__ constexpr bool kb_is_dir(int s, int kb, bool v = true) { return v && s == 9 && kb == 4; }
-__host__ __device__ constexpr int kb_act_index(int s, int kb) { return s == 5 ? kb - 1 : kb; }
 __host__ __device__ constexpr int tc_slabs_per_tile(bool v = true, bool t = false) {
   int n = 0;
   for (int s = 0; s < tc_steps(v); ++s) n += step_nkb(s, v, t);
@@ -297,30 +294,13 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
   for (int i = threadIdx.x; i < TC_CONST_FLOATS; i += C::THREADS) s_const[i] = __ldg(P.consts + i);
   const long long my_tiles = blockIdx.x < P.n_tiles ? (P.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
   const uint32_t total = (uint32_t)(my_tiles * SLABS);
-  // Refills: the warpgroup that releases a slot second issues the slab NSLOT places further on, right away.  A
-  // per-slot release counter in place of an `empty` barrier decides which one that is, so neither warpgroup ever waits
-  // for the other's release: warpgroup 0 keeps issuing MMAs on the slabs already in the ring while warpgroup 1 is behind
-  // (e.g. in its epilogue), and the other way round.
-  const uint32_t rel = sbase + C::OFF_BAR + 8 * C::NSLOT;          // NSLOT release counters (u32)
-  auto refill = [&](uint32_t qq) {
+  auto fill = [&](uint32_t qq) {                        // the slab of fill qq, in consumption order
     const uint32_t j = qq % SLABS, off = P.plan.lin_off[j], bytes = P.plan.lin_off[j + 1] - off;
     mbar_arrive_expect_tx(R.full(qq), bytes);
     bulk_g2s(R.slot(qq), P.wimg + off, bytes, R.full(qq));
   };
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < C::NSLOT; ++i) {
-      mbar_init(R.full(i), 1);
-      st_shared_u32(rel + 4 * i, 0);
-    }
-    fence_mbar_init();
-    for (uint32_t i = 0; i < C::NSLOT && i < total; ++i) refill(i);
-  }
+  if (threadIdx.x == 0) R.init(total, fill);
   __syncthreads();
-  auto release = [&](uint32_t qq) {
-    // acq_rel: the first releaser's finished MMA reads of the slot are ordered before the second one's refill
-    if (wtid == 0 && qq + C::NSLOT < total && (atom_add_acq_rel_cta(rel + 4 * (qq % C::NSLOT), 1) & 1)) refill(qq + C::NSLOT);
-    __syncwarp();
-  };
 
   const float4 ob = *reinterpret_cast<const float4*>(s_const + TC_CONST_OUT);
   float d[128];
@@ -372,94 +352,70 @@ __device__ __forceinline__ void mlp_tc_body(const TcParams& P) {
       wg_sync(wg);
     }
     float alpha[2] = {0.f, 0.f};
-    // rendering: unrolled, so each step's k-blocks and epilogue touch a fixed part of `a` and only that part is live
+    // rendering: unrolled, so each step's k-blocks and epilogue touch a fixed part of `a` and only that part is live (the
+    // training kernels do not hold `a`: the unrolled loop makes them spill)
 #pragma unroll (kTrain ? 1 : STEPS)
     for (int s = 0; s < STEPS; ++s) {
       const int nkb = step_nkb(s, kView, kTime);
+      const bool wide = s <= (kView ? 8 : 7), views = kView && s == 9;     // N = 256 / 128 (views) / 16 (output)
       wgmma_fence();
-      if constexpr (kTrain) {
-        // training forward: every k-block's A operand from shared memory (the activation blocks are the stash's source;
-        // holding `a` as well makes these kernels spill)
-        for (int kb = 0; kb < nkb; ++kb) {
-          const uint32_t qq = qbase + kb;
-          R.wait_full(qq);
-          const bool time = kb_is_time(s, kb, kTime);
-          const uint32_t a_addr = kb_is_pos(s, kb, kView, kTime) ? wbase + C::OFF_POS
-                                : (kb_is_dir(s, kb, kView) || time) ? wbase + C::OFF_DIR
-                                                   : wbase + kb_act_index(s, kb) * TC_KB_BYTES;
-          // K advances by 32 B (= 2 in descriptor address units) inside the 128-byte swizzle atom; a bias slab is one
-          // K = 16 MMA on the last K slice (channels 48..63 of the position encoding x columns 48..63 of the slab), a time
-          // slab two on K slices 2..3 (channels 32..63 of the direction block)
-          const bool bias = kb_is_bias(s, kb, kView);
-          const int k0 = bias ? 3 : (time ? 2 : 0), k1 = kb_is_dir(s, kb, kView) ? 2 : 4;
-          const uint64_t a_desc = gmma_desc_k(a_addr), b_desc = gmma_desc_k(R.slot(qq));
+      int kb = 0;
+      // one k-block: wait for its slab, issue its MMAs (`issue(b_desc, first k-block of the step)`), commit, and
+      // release the previous k-block's slab once its MMAs have retired
+      auto kblock = [&](auto&& issue) {
+        const uint32_t qq = qbase + kb;
+        R.wait_full(qq);
+        issue(gmma_desc_k(R.slot(qq)), kb == 0);
+        wgmma_commit();
+        if (kb > 0) { wgmma_wait<1>(); R.release(qq - 1, total, fill); }
+        ++kb;
+      };
+      // a k-block whose A operand is a block in shared memory, K slices k0..k1-1.  K advances by 32 B (= 2 in descriptor
+      // address units) inside the 128-byte swizzle atom.
+      auto smem_kblock = [&](uint32_t a_addr, int k0, int k1) {
+        kblock([&](uint64_t b_desc, bool first) {
+          const uint64_t a_desc = gmma_desc_k(a_addr);
           for (int k = k0; k < k1; ++k) {
-            const uint32_t acc = (kb | (k - k0)) != 0;
-            if (s <= (kView ? 8 : 7)) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
-            else if (kView && s == 9) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+            const uint32_t acc = !first || k > k0;
+            if (wide) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
+            else if (views) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
             else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
           }
-          wgmma_commit();
-          if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
-        }
-      } else {
-        const bool wide = s <= (kView ? 8 : 7), views = kView && s == 9;     // N = 256 / 128 (views) / 16 (output)
-        int kb = 0;
-        // one k-block: wait for its slab, issue its MMAs (`issue(b_desc, first k-block of the step)`), commit, and
-        // release the previous k-block's slab once its MMAs have retired
-        auto kblock = [&](auto&& issue) {
-          const uint32_t qq = qbase + kb;
-          R.wait_full(qq);
-          issue(gmma_desc_k(R.slot(qq)), kb == 0);
-          wgmma_commit();
-          if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
-          ++kb;
-        };
-        // a k-block whose A operand is an encoding block in shared memory, K slices k0..k1-1.  K advances by 32 B (= 2
-        // in descriptor address units) inside the 128-byte swizzle atom.
-        auto smem_kblock = [&](uint32_t a_addr, int k0, int k1) {
-          kblock([&](uint64_t b_desc, bool first) {
-            const uint64_t a_desc = gmma_desc_k(a_addr);
-            for (int k = k0; k < k1; ++k) {
-              const uint32_t acc = !first || k > k0;
-              if (wide) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, acc);
-              else if (views) wgmma_n128(d, a_desc + 2 * k, b_desc + 2 * k, acc);
-              else wgmma_n16(d16, a_desc + 2 * k, b_desc + 2 * k, acc);
-            }
-          });
-        };
-        if (s == 0 || s == 5) smem_kblock(wbase + C::OFF_POS, 0, 4);       // position encoding (step 5: "input first", :131)
-        if (s > 0) {
-          const int nact = kView && s == LAST ? 2 : 4;                      // rgb reads the 128 columns of the views layer
+        });
+      };
+      if (s == 0 || s == 5) smem_kblock(wbase + C::OFF_POS, 0, 4);       // position encoding (step 5: "input first", :131)
+      if (s > 0) {
+        const int nact = kView && s == LAST ? 2 : 4;                      // rgb reads the 128 columns of the views layer
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (j < nact) {
-              kblock([&](uint64_t b_desc, bool first) {
+        for (int j = 0; j < 4; ++j) {
+          if (j < nact) {
+            // training: the activation block in shared memory (the source of the stash's stores); rendering: `a`
+            if constexpr (kTrain) smem_kblock(wbase + j * TC_KB_BYTES, 0, 4);
+            else kblock([&](uint64_t b_desc, bool first) {
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const uint32_t* f = a + 16 * j + 4 * k;
-                  const uint32_t acc = !first || k > 0;
-                  if (wide) wgmma_n256_rs(d, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
-                  else if (views) wgmma_n128_rs(d, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
-                  else wgmma_n16_rs(d16, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
-                }
-              });
-            }
+              for (int k = 0; k < 4; ++k) {
+                const uint32_t* f = a + 16 * j + 4 * k;
+                const uint32_t acc = !first || k > 0;
+                if (wide) wgmma_n256_rs(d, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
+                else if (views) wgmma_n128_rs(d, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
+                else wgmma_n16_rs(d16, f[0], f[1], f[2], f[3], b_desc + 2 * k, acc);
+              }
+            });
           }
         }
-        // the trailing k-block: a bias slab is one K = 16 MMA on the last K slice (channels 48..63 of the position
-        // encoding x columns 48..63 of the slab), the direction encoding two on K slices 0..1, a time slab two on K
-        // slices 2..3 (channels 32..63 of the direction block)
-        if (kb < nkb) {
-          if (kb_is_bias(s, kb, kView)) smem_kblock(wbase + C::OFF_POS, 3, 4);
-          else if (kb_is_dir(s, kb, kView)) smem_kblock(wbase + C::OFF_DIR, 0, 2);
-          else smem_kblock(wbase + C::OFF_DIR, 2, 4);
-        }
+      }
+      // the trailing k-block: a bias slab is one K = 16 MMA on the last K slice (channels 48..63 of the position
+      // encoding x columns 48..63 of the slab), the direction encoding two on K slices 0..1, a time slab two on K
+      // slices 2..3 (channels 32..63 of the direction block)
+      if (kb < nkb) {
+        if (kb_is_bias(s, kb, kView)) smem_kblock(wbase + C::OFF_POS, 3, 4);
+        else if (kb_is_dir(s, kb, kView)) smem_kblock(wbase + C::OFF_DIR, 0, 2);
+        else smem_kblock(wbase + C::OFF_DIR, 2, 4);
       }
       wgmma_wait<0>();
       wgmma_fence_regs(d);
       wgmma_fence_regs(d16);
-      release(qbase + nkb - 1);
+      R.release(qbase + nkb - 1, total, fill);
       qbase += nkb;
       if (s < LAST) {
         // training forward: the MMAs of this step read the activation blocks, the stash stores of the previous step

@@ -137,24 +137,12 @@ __device__ __forceinline__ void mlp_tc_bwd_body(const BwParams& P) {
   }
   const long long my_tiles = blockIdx.x < P.n_tiles ? (P.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
   const uint32_t total = (uint32_t)(my_tiles * SLABS);
-  uint32_t pq = 0;                                   // producer (thread 0): next slab to issue
-  auto produce = [&]() {
-    if (pq >= total) return;
-    if (pq >= C::NSLOT) mbar_wait(R.empty(pq), (pq / C::NSLOT - 1) & 1);
-    mbar_arrive_expect_tx(R.full(pq), TC_SLAB_BYTES);
-    bulk_g2s(R.slot(pq), P.wimg + (size_t)(pq % SLABS) * TC_SLAB_BYTES, TC_SLAB_BYTES, R.full(pq));
-    ++pq;
+  auto fill = [&](uint32_t qq) {
+    mbar_arrive_expect_tx(R.full(qq), TC_SLAB_BYTES);
+    bulk_g2s(R.slot(qq), P.wimg + (size_t)(qq % SLABS) * TC_SLAB_BYTES, TC_SLAB_BYTES, R.full(qq));
   };
-  if (threadIdx.x == 0) {
-    R.init();
-    for (int i = 0; i < C::NSLOT; ++i) produce();
-  }
+  if (threadIdx.x == 0) R.init(total, fill);
   __syncthreads();
-  auto release = [&](uint32_t qq) {
-    if (wtid == 0) mbar_arrive_local(R.empty(qq));
-    if (threadIdx.x == 0) produce();
-    __syncwarp();
-  };
   const float S = __ldg(P.scale);
 
   float d[128];
@@ -237,11 +225,11 @@ __device__ __forceinline__ void mlp_tc_bwd_body(const BwParams& P) {
 #pragma unroll
         for (int k = 0; k < 4; ++k) wgmma_n256(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
         wgmma_commit();
-        if (kb > 0) { wgmma_wait<1>(); release(qq - 1); }
+        if (kb > 0) { wgmma_wait<1>(); R.release(qq - 1, total, fill); }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(d);
-      release(qbase + nkb - 1);
+      R.release(qbase + nkb - 1, total, fill);
       qbase += nkb;
       if (wtid == 0) tma_store_wait_read();
       wg_sync(wg);

@@ -40,9 +40,6 @@ __device__ __forceinline__ uint32_t atom_add_acq_rel_cta(uint32_t addr, uint32_t
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_local(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar) : "memory");
@@ -222,19 +219,35 @@ __device__ __forceinline__ void tma_store_rows(const CUtensorMap* map, uint32_t 
   tma_store_commit();
 }
 
-// One warpgroup's view of an NSLOT-deep weight ring: the slabs of a launch are consumed in a fixed order by both warpgroups;
-// a slab's slot is refilled once both have released it.  In the backward chain thread 0 of the CTA is the producer: it issues
-// the first NSLOT slabs and, after each of its own releases, waits on `empty` and issues the slab NSLOT places further on.
-// The forward kernel (mlp_tc.cu) uses the slots and `full` barriers only: there the second releaser refills.
-template <int NSLOT>
+// An NSLOT-deep ring of SLOT_BYTES slots, shared by the CTA's two warpgroups: fills 0 .. total - 1 of a launch are consumed
+// in a fixed order by both, and each warpgroup releases each fill once its MMAs on it have retired (the last NSLOT fills
+// need no release).  The warpgroup that
+// releases a slot second refills it, right away, with the fill NSLOT places further on.  A per-slot release counter in place
+// of an `empty` barrier decides which one that is, so neither warpgroup ever waits for the other's release: one keeps
+// issuing MMAs on the fills already in the ring while the other is behind (e.g. in its epilogue).
+// `fill(q)` (one thread) announces fill q's bytes on full(q) and starts its copies into slot(q).
+template <int NSLOT, uint32_t SLOT_BYTES = TC_SLAB_BYTES>
 struct TcRing {
-  uint32_t ring, bar;       // shared addresses: NSLOT slots of TC_SLAB_BYTES; full[NSLOT] then empty[NSLOT]
-  __device__ uint32_t slot(uint32_t q) const { return ring + (q % NSLOT) * TC_SLAB_BYTES; }
+  uint32_t ring, bar;       // shared addresses: NSLOT slots; full barriers [NSLOT] (8 B), then release counters [NSLOT] (u32)
+  __device__ uint32_t slot(uint32_t q) const { return ring + (q % NSLOT) * SLOT_BYTES; }
   __device__ uint32_t full(uint32_t q) const { return bar + 8 * (q % NSLOT); }
-  __device__ uint32_t empty(uint32_t q) const { return bar + 8 * (NSLOT + q % NSLOT); }
   __device__ void wait_full(uint32_t q) const { mbar_wait(full(q), (q / NSLOT) & 1); }
-  __device__ void init() const {
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(bar + 8 * i, 1); mbar_init(bar + 8 * (NSLOT + i), 2); }
+  // one thread, before the CTA's first barrier: barriers, counters and the first NSLOT fills
+  template <class Fill>
+  __device__ void init(uint32_t total, Fill&& fill) const {
+    for (int i = 0; i < NSLOT; ++i) {
+      mbar_init(full(i), 1);
+      st_shared_u32(bar + 8 * NSLOT + 4 * i, 0);
+    }
     fence_mbar_init();
+    for (uint32_t i = 0; i < NSLOT && i < total; ++i) fill(i);
+  }
+  // the calling warp's warpgroup is done with fill q
+  template <class Fill>
+  __device__ void release(uint32_t q, uint32_t total, Fill&& fill) const {
+    // acq_rel: the first releaser's finished MMA reads of the slot are ordered before the second one's refill
+    if ((threadIdx.x & 127) == 0 && q + NSLOT < total && (atom_add_acq_rel_cta(bar + 8 * NSLOT + 4 * (q % NSLOT), 1) & 1))
+      fill(q + NSLOT);
+    __syncwarp();
   }
 };

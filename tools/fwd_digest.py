@@ -1,12 +1,15 @@
-"""Bit-for-bit comparison of the tensor-core MLP forward and the frame drivers between two builds of the library.
+"""Bit-for-bit comparison of the tensor-core MLP forward and backward chain and the frame drivers between two builds of the
+library.
 
     python tools/fwd_digest.py dump OUT.json [--root TREE]     # run TREE's library (default: this tree) on seeded inputs
     python tools/fwd_digest.py compare A.json B.json           # exit 1 unless every record is identical
 
 `dump` runs the tensor-core forward on seeded inputs and records a SHA-256 of every output buffer: the training forward's raw,
-activation stash (st_x, st_f, st_v) and sign words, and the inference raw in per-sample, per-ray-view and fused ray modes,
-for view-dependent nets (posenc and rotate), a view-independent net (no st_f / st_v, 8 sign-word planes) and a NeRF-T net
-([n,4] points; no fused ray mode, which NeRF-T slots do not take).  Sizes
+activation stash (st_x, st_f, st_v) and sign words, the backward chain's gradient planes (nm_mlp_backward on that stash with a
+seeded d_raw and a fixed loss scale: g_pre, g_f, g_v), and the inference raw in per-sample, per-ray-view and fused ray modes,
+for view-dependent nets (posenc and rotate), a view-independent net (no st_f / st_v / g_f / g_v, 8 sign-word planes) and a
+NeRF-T net ([n,4] points; no fused ray mode, which NeRF-T slots do not take).  The weight-gradient GEMM (nm_dw_gemm) is not
+recorded: it sums across CTAs with red.global.add, so its output's last bits vary from run to run.  Sizes
 cover ragged tiles, several waves of the persistent grid and a frame-sized ray chunk.  Its frames section renders with
 every driver (vanilla coarse-only and coarse + fine, smpl_nerf canonical and posed, hybrid, multi-person with 2 and 3
 actors), each with host and device output, a pixel range and a pixel list, the default chunk and a ragged one, and
@@ -62,6 +65,17 @@ def dump(out, root):
                 (("raw", raw), ("st_x", sx), ("st_m", sm))
             for k, v in outs:
                 res[f"{name}/train/n={n}/{k}"] = _digest(v)
+            # backward chain on that stash, loss scale 2^6 (max |d_raw| * S about 256, as autograd picks it)
+            d_raw = torch.randn(n, 4, device=dev, generator=g)
+            scale = torch.full((1,), 64.0, device=dev)
+            gp = torch.empty(8, n, 256, device=dev, dtype=torch.float16)
+            gf = torch.empty(n, 256, device=dev, dtype=torch.float16) if view else None
+            gv = torch.empty(n, 128, device=dev, dtype=torch.float16) if view else None
+            ctx.check(ctx.lib.nm_mlp_backward(ctx.h, slot, _p(d_raw), _p(scale), n, _p(sv if view else None), _p(sm), _p(gp),
+                                              _p(gf), _p(gv), ctx.stream()))
+            torch.cuda.synchronize()
+            for k, v in (("g_pre", gp), ("g_f", gf), ("g_v", gv)) if view else (("g_pre", gp),):
+                res[f"{name}/backward/n={n}/{k}"] = _digest(v)
             # inference, per-sample views and one view row per 7 samples (n rounded down to a multiple of 7)
             for group in (0,) if time else (0, 7):
                 m = n if group == 0 else n - n % group
