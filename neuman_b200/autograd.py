@@ -59,6 +59,32 @@ def _mm32(a, b):
     return torch.mm(a, b, out_dtype=torch.float32)
 
 
+def _bmm32(a, b):
+    return torch.bmm(a, b, out_dtype=torch.float32)
+
+
+_K_CHUNK = 4096         # rows per batch of the K = n weight-gradient GEMMs (_wgrad)
+
+
+def _wgrad(G, X):
+    """G^T @ X over the n rows of G [n, M] and X [n, N] (fp16, row-major) -> fp32 [M, N]: a K = n weight-gradient GEMM.
+    One torch.mm with K = n leaves it to cuBLAS to split K, and for some shapes (n ~ 14 000 - 40 000 with 64- or 96-wide
+    X on an H100) the kernel it picks reduces the split below fp32: up to 1.5 times the error bound of any fp32
+    summation order (tests/dw_exact.py gemm_window_any_order; DESIGN.md §2).  So K is split here: a batched GEMM over
+    whole _K_CHUNK-row blocks, which fills the GPU without a split of its own, the fp32 sum of its partials, and the
+    remaining rows as one GEMM with K < _K_CHUNK."""
+    n = G.shape[0]
+    nb = n // _K_CHUNK
+    k = nb * _K_CHUNK
+    out = None
+    if nb:
+        out = _bmm32(G[:k].view(nb, _K_CHUNK, G.shape[1]).transpose(1, 2), X[:k].view(nb, _K_CHUNK, X.shape[1])).sum(0)
+    if n > k:
+        t = _mm32(G[k:].t(), X[k:])
+        out = t if out is None else out + t
+    return out
+
+
 class _JoinerMLP(torch.autograd.Function):
     """forward: k_mlp_tc<.., kTrain> (csrc/mlp_tc.cu) = the inference kernel + an fp16 stash of every layer
     output and the ReLU sign words.
@@ -177,9 +203,9 @@ def _encodings(joiner, pts, views):
 def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
     """dW = g^T @ layer input, K = n, fp16 operands / fp32 accumulate; g_* carry the loss scale 1/inv.
     The nine 256-wide GEMMs and their bias gradients are one k_dw_gemm launch (csrc/dw_gemm.cu).  The narrow ones
-    (encodings, dL/d raw) go through cuBLAS with whole 16-byte aligned planes as operands (the 64-/32-channel
-    encodings including their padding, the [n,8]-padded dL/d raw: 63-/27-wide slices made cuBLAS fall back to an
-    sm_75 kernel); the position stash's constant-1.0 channel returns pts_linears.0's bias gradient as GEMM column 63."""
+    (encodings, dL/d raw) go through cuBLAS with K split into fixed blocks (_wgrad) and whole 16-byte aligned planes
+    as operands (the 64-/32-channel encodings including their padding, the [n,8]-padded dL/d raw: 63-/27-wide slices
+    made cuBLAS fall back to an sm_75 kernel); the position stash's constant-1.0 channel returns pts_linears.0's bias gradient as GEMM column 63."""
     sx, sf, sv, _ = stash
     spe, sdpe = _encodings(joiner, pts, views)
     ctx = _ctx_for(g)
@@ -187,22 +213,21 @@ def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
     grads = {}
     g8 = torch.zeros(g.shape[0], 8, device=g.device, dtype=torch.float16)
     g8[:, :4] = g * (1.0 / inv)
-    g8t = g8.t()
     if ops.is_viewless(joiner):
         # output_linear (models/vanilla.py:146) reads layer 7's output: g^T @ X7 in cuBLAS, as alpha_linear below
-        grads['output_linear.weight'] = _mm32(g8t, sx[7])[:4] * inv
+        grads['output_linear.weight'] = _wgrad(g8, sx[7])[:4] * inv
         grads['output_linear.bias'] = g.sum(0)
     else:
         n_dpe = joiner.dir_pe.out_dim                                     # 27
-        grads['rgb_linear.weight'] = _mm32(g8t, sv)[:3] * inv
+        grads['rgb_linear.weight'] = _wgrad(g8, sv)[:3] * inv
         grads['rgb_linear.bias'] = g[:, :3].sum(0)
-        grads['alpha_linear.weight'] = _mm32(g8t, sx[7])[3:4] * inv
+        grads['alpha_linear.weight'] = _wgrad(g8, sx[7])[3:4] * inv
         grads['alpha_linear.bias'] = g[:, 3].sum().reshape(1)
-    w0 = _mm32(g_pre[0].t(), spe) * inv                                   # [256,64]: column 63 (84) = bias gradient (1.0 channel)
+    w0 = _wgrad(g_pre[0], spe) * inv                                   # [256,64]: column 63 (84) = bias gradient (1.0 channel)
     dw, db = _dw_kernel(ctx, g_pre, g_f, g_v, sx, sf, g.shape[0])
     dw, db = dw * inv, db * inv
     if sdpe is not None:
-        wd = _mm32(g_v.t(), sdpe) * inv                                   # [128, 32]
+        wd = _wgrad(g_v, sdpe) * inv                                   # [128, 32]
         grads['views_linears.0.weight'] = torch.cat([dw[8, :128], wd[:, :n_dpe]], 1)
         grads['views_linears.0.bias'] = db[8, :128]
         grads['feature_linear.weight'], grads['feature_linear.bias'] = dw[7], db[7]
@@ -210,7 +235,7 @@ def _weight_grads(joiner, stash, pts, views, g, g_pre, g_f, g_v, inv):
         if l == 0:
             w = w0[:, :n_pe]
         elif l == 5:
-            w = torch.cat([_mm32(g_pre[5].t(), spe)[:, :n_pe] * inv, dw[4]], 1)
+            w = torch.cat([_wgrad(g_pre[5], spe)[:, :n_pe] * inv, dw[4]], 1)
         else:
             w = dw[l - 1]
         grads['pts_linears.%d.weight' % l] = w
